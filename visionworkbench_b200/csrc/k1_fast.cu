@@ -7,18 +7,23 @@
 // dx-minor order => first disparity wins ties; all-equal => invalid), so it is bit-identical to the
 // reference while doing ~10 issue slots per (pixel, disparity) instead of ~70 bytes of DRAM traffic.
 //
-// Decomposition (persistent CTAs of 4 warps, one CTA per SM; work item = 236-column x 32-row band):
+// Decomposition (persistent CTAs of 8 warps, one CTA per SM; work item = 236-column x th-row band, th chosen by
+// fast_geom within the shared-memory budget -- up to 61 rows at 128 x 128 / 21 x 21):
 //   * values are pre-packed (pack kernels) as u16 (v-vmin)*8, one contiguous row per strip, so that a
 //     lane fetches its 8 left / 16 right columns with conflict-free 16-byte LDS.128 loads
-//   * the left tile (32+ky-1 rows) and a ring of right rows are staged in shared memory with TMA bulk
+//   * the left tile (th+ky-1 rows) and a ring of right rows are staged in shared memory with TMA bulk
 //     copies (cp.async.bulk + mbarrier); one new right row is prefetched per dy while the CTA computes
+//   * warp w takes the dx octets w, w+8, ... and slides each over every row of the band, so the ky rows
+//     that seed its vertical sums are summed once per (dy, octet) and band
 //   * lane l owns padded columns 8l..8l+7 and 8 consecutive dx: V[8][8] vertical sliding sums live in
 //     registers (VABSDIFF accumulate: +new row, -old row)
 //   * the kx-wide horizontal sums are formed without shared memory: in-lane prefix sums + 9 warp
 //     shuffles per 8 outputs (blocked-prefix scheme), 3-input IADD3
 //   * arg-best: costs are pre-scaled by 8 so key = cost*8 + b; min over the 8 dx is 7 VIADDMNMX;
-//     the running best (cost only) sits in shared memory, the index goes to a global scratch plane
-//     on the (rare) improvements; warps cover disjoint dx subsets and are merged at the end of the band
+//     one shared-memory plane holds a 64-bit key (cost << 32 | raster index) per band pixel.  The hot
+//     loop reads only the high words; the (rare) candidates with a cost <= the stored one go through a
+//     64-bit atomicMin, so the lowest cost and, among equal costs, the first disparity in raster order
+//     wins whichever warp reaches it first
 //   * pixels whose arg-best is disparity (0,0) are re-checked by a small kernel for the
 //     "every disparity gave the same cost => invalid" rule (Correlation.cc:121-133)
 #include "k1_fast_common.cuh"
@@ -69,6 +74,33 @@ int image_stats_launch(ImgF img, float* d_result3, cudaStream_t st) {
   return VWB200_OK;
 }
 
+// ---- band geometry ------------------------------------------------------------------------------------------------
+static constexpr int FK_TH_MAX = 64;                 // tallest band considered (the headline fits 61 rows)
+static constexpr size_t FK_SMEM = 227 * 1024;
+static constexpr uint32_t FK_INIT_HI = 0x7fffffffu;  // high word of an empty key: above every (cost*8 | 7)
+
+// key plane [th][256] (u64) | left tile [th+ky-1][256] (u16) | right ring [th+ky][rw] (u16) | 2 mbarriers
+static size_t fast_smem_bytes(const FastGeom& g) {
+  return (size_t)g.th * F_COLS * 8 + (size_t)g.ltile_rows * F_COLS * 2 + (size_t)g.ring_slots * g.rw * 2 + 64;
+}
+
+// Band height: a taller band spreads the seeding of each (dy, octet) -- ky rows of vertical sums plus a first row
+// without the sliding update, about 0.15*ky row steps -- over more rows, but makes fewer, longer work items.  Take
+// the height between F_TH and what the shared memory holds with the least estimated time: waves of work items x
+// row steps per item (make_geom picks the dy chunking J for each height).
+static FastGeom fast_geom(int W, int H, int sx, int sy, int kx, int ky) {
+  FastGeom best = make_geom(W, H, sx, sy, kx, ky, F_TH);
+  double tbest = -1.0;
+  for (int th = F_TH; th <= FK_TH_MAX; ++th) {
+    const FastGeom g = make_geom(W, H, sx, sy, kx, ky, th);
+    if (fast_smem_bytes(g) > FK_SMEM) break;
+    const long long waves = ((long long)g.NS * g.NB * g.J + kNumSMs - 1) / kNumSMs;
+    const double t = (double)waves * g.dy_per * ((th < H ? th : H) + 0.15 * ky) * (1.0 + 0.004 * (g.J - 1));
+    if (tbest < 0.0 || t < tbest) { tbest = t; best = g; }
+  }
+  return best;
+}
+
 int k1_fast_supported(int cost, int kx, int ky, int sx, int sy, float vmin, float vmax, bool integer_valued) {
   if (cost != VWB200_ABSOLUTE_DIFFERENCE && cost != VWB200_SQUARED_DIFFERENCE) return VWB200_ENOIMPL;
   if (!integer_valued) return VWB200_ENOIMPL;
@@ -83,18 +115,16 @@ int k1_fast_supported(int cost, int kx, int ky, int sx, int sy, float vmin, floa
   if (sx < F_B || sx > 512 || sy < 1) return VWB200_ENOIMPL;
   if ((long long)sx * sy > 65536) return VWB200_ENOIMPL;
   if ((long long)sx * sy < 64) return VWB200_ENOIMPL;      // tiny searches: the generic kernel is as good
-  FastGeom g = make_geom(256, 32, sx, sy, kx, ky);
-  if (fast_smem_bytes(g) > 227 * 1024) return VWB200_ENOIMPL;
+  if (fast_smem_bytes(make_geom(256, F_TH, sx, sy, kx, ky, F_TH)) > FK_SMEM) return VWB200_ENOIMPL;
   return VWB200_OK;
 }
 
 size_t k1_fast_workspace_bytes(int W, int H, int sx, int sy, int kx, int ky) {
-  FastGeom g = make_geom(W, H, sx, sy, kx, ky);
+  FastGeom g = fast_geom(W, H, sx, sy, kx, ky);
   size_t l = (size_t)g.NS * g.lrows * F_COLS * 2;
   size_t r = (size_t)g.NS * g.rrows * g.rw * 2;
-  size_t idx = (size_t)1024 * F_SUBSETS * F_TH * F_COLS * 2;    // per-CTA index planes (<= 1024 CTAs)
   size_t part = g.J > 1 ? (size_t)g.J * W * H * 6 + 64 : 0;      // per-dy-chunk partial (cost u32, index u16)
-  return l + r + idx + part + 512;
+  return l + r + part + 512;
 }
 
 // ---- pack kernels: float raster -> u16 (v - vmin) * 4 in the lane-transposed strip layout ------------
@@ -159,14 +189,21 @@ __device__ __forceinline__ void load_row_f(const uint16_t* lrow, const uint16_t*
 #pragma unroll
   for (int i = 0; i < 8; ++i) Rv[8 + i] = t[i];
 }
+// High word of a pixel's key in the shared plane (the hot loop compares costs only).
+__device__ __forceinline__ uint32_t key_hi(const unsigned long long* k) { return reinterpret_cast<const uint32_t*>(k)[1]; }
+// A candidate: keep the lower cost and, for equal costs, the lower raster index (= the first disparity).
+__device__ __forceinline__ void offer_key(unsigned long long* k, uint32_t hi, uint32_t idx) {
+  atomicMin(k, ((unsigned long long)hi << 32) | idx);
+}
+
 template <int KX, bool FSEED, bool FULL>
 __device__ __forceinline__ void fast_pass(const uint16_t* __restrict__ ltile, const uint16_t* __restrict__ rring,
-                                          uint32_t* __restrict__ state, uint16_t* __restrict__ idxp,
-                                          int lane, int g, int ky, int ring_slots, int rw, int ring_base, int idx_base, int row0, int nb) {
+                                          unsigned long long* __restrict__ keys,
+                                          int lane, int g, int ky, int ring_slots, int rw, int ring_base, int idx_base, int nrows, int nb) {
   int V[8][F_B];
-  const uint16_t* lp = ltile + row0 * F_COLS + 8 * lane;       // + row*256            (16-byte aligned)
+  const uint16_t* lp = ltile + 8 * lane;                       // + row*256            (16-byte aligned)
   const uint16_t* rp = rring + 8 * (lane + g);                 // + slot*rw            (16-byte aligned)
-  int slot_new = ring_base;                                     // ring slot of right row (dy + row0 + t)
+  int slot_new = ring_base;                                     // ring slot of right row (dy + t)
   // ---- seed: first ky rows.  The integer main loop is bound by the ALU pipe (VABSDIFF), so the seed
   //      rows are summed in fp32 on the otherwise idle FMA pipes (exact: sums < 2^23) and converted once.
   if (FSEED) {
@@ -204,7 +241,7 @@ __device__ __forceinline__ void fast_pass(const uint16_t* __restrict__ ltile, co
     }
   }
   int slot_old = ring_base;
-  for (int y = 0; y < F_RH; ++y) {
+  for (int y = 0; y < nrows; ++y) {
     if (y > 0) {
       {
         int Lv[8], Rv[16];
@@ -238,20 +275,17 @@ __device__ __forceinline__ void fast_pass(const uint16_t* __restrict__ ltile, co
 #pragma unroll
       for (int r = 0; r < 8; ++r) m[r] = (b == 0) ? o[r] : min(o[r] + b, m[r]);
     }
-    // ---- running best (shared memory), index plane (global) on improvement ----
-    uint32_t* srow = state + y * F_COLS + lane;
+    // ---- running best: high words hold cost*8 | 7, so m <= s <=> cost <= best cost.  Equal costs are candidates
+    //      too: another warp may hold the same cost at a later disparity ----
+    unsigned long long* krow = keys + y * F_COLS + lane;
     uint32_t s8[8];
-    bool improved = false;
+    bool cand = false;
 #pragma unroll
-    for (int r = 0; r < 8; ++r) { s8[r] = srow[r * 32]; improved |= ((uint32_t)m[r] < s8[r]); }
-    if (improved) {            // rare once the search has seen the neighbourhood of the true match
+    for (int r = 0; r < 8; ++r) { s8[r] = key_hi(krow + r * 32); cand |= ((uint32_t)m[r] <= s8[r]); }
+    if (cand) {                // rare once the search has seen the neighbourhood of the true match
 #pragma unroll
-      for (int r = 0; r < 8; ++r) {
-        if ((uint32_t)m[r] < s8[r]) {
-          srow[r * 32] = (uint32_t)m[r] & ~7u;
-          idxp[y * F_COLS + r * 32 + lane] = (uint16_t)(idx_base + (m[r] & 7));
-        }
-      }
+      for (int r = 0; r < 8; ++r)
+        if ((uint32_t)m[r] <= s8[r]) offer_key(krow + r * 32, (uint32_t)m[r] | 7u, (uint32_t)(idx_base + (m[r] & 7)));
     }
   }
 }
@@ -262,14 +296,14 @@ __device__ __forceinline__ void fast_pass(const uint16_t* __restrict__ ltile, co
 // leave room for the key trick, so the arg-min over the octet is tracked with compare/select.
 template <int KX>
 __device__ __forceinline__ void fast_pass_sq(const uint16_t* __restrict__ ltile, const uint16_t* __restrict__ rring,
-                                             uint32_t* __restrict__ state, uint16_t* __restrict__ idxp,
-                                             int lane, int g, int ky, int ring_slots, int rw, int ring_base, int idx_base, int row0, int nb) {
+                                             unsigned long long* __restrict__ keys,
+                                             int lane, int g, int ky, int ring_slots, int rw, int ring_base, int idx_base, int nrows, int nb) {
   int V[8][F_B];
 #pragma unroll
   for (int a = 0; a < 8; ++a)
 #pragma unroll
     for (int b = 0; b < F_B; ++b) V[a][b] = 0;
-  const uint16_t* lp = ltile + row0 * F_COLS + 8 * lane;
+  const uint16_t* lp = ltile + 8 * lane;
   const uint16_t* rp = rring + 8 * (lane + g);
   int slot_new = ring_base;
   for (int t = 0; t < ky; ++t) {
@@ -282,7 +316,7 @@ __device__ __forceinline__ void fast_pass_sq(const uint16_t* __restrict__ ltile,
     if (++slot_new == ring_slots) slot_new = 0;
   }
   int slot_old = ring_base;
-  for (int y = 0; y < F_RH; ++y) {
+  for (int y = 0; y < nrows; ++y) {
     if (y > 0) {
       {
         int Lv[8], Rv[16];
@@ -320,14 +354,10 @@ __device__ __forceinline__ void fast_pass_sq(const uint16_t* __restrict__ ltile,
         else if (c < m[r]) { m[r] = c; mb[r] = b; }
       }
     }
-    uint32_t* srow = state + y * F_COLS + lane;
+    unsigned long long* krow = keys + y * F_COLS + lane;      // high words: the uint32 cost
 #pragma unroll
-    for (int r = 0; r < 8; ++r) {
-      if (m[r] < srow[r * 32]) {
-        srow[r * 32] = m[r];
-        idxp[y * F_COLS + r * 32 + lane] = (uint16_t)(idx_base + mb[r]);
-      }
-    }
+    for (int r = 0; r < 8; ++r)
+      if (m[r] <= key_hi(krow + r * 32)) offer_key(krow + r * 32, m[r], (uint32_t)(idx_base + mb[r]));
   }
 }
 
@@ -364,14 +394,14 @@ __device__ __forceinline__ void window_sums_f(const float (&p)[8], float (&out)[
 
 template <int KX>
 __device__ __forceinline__ void fast_pass_f(const uint16_t* __restrict__ ltile, const uint16_t* __restrict__ rring,
-                                            float* __restrict__ state, uint16_t* __restrict__ idxp,
-                                            int lane, int g, int ky, int ring_slots, int rw, int ring_base, int idx_base, int row0) {
+                                            unsigned long long* __restrict__ keys,
+                                            int lane, int g, int ky, int ring_slots, int rw, int ring_base, int idx_base, int nrows) {
   float V[8][F_B];
 #pragma unroll
   for (int a = 0; a < 8; ++a)
 #pragma unroll
     for (int b = 0; b < F_B; ++b) V[a][b] = 0.0f;
-  const uint16_t* lp = ltile + row0 * F_COLS + 8 * lane;
+  const uint16_t* lp = ltile + 8 * lane;
   const uint16_t* rp = rring + 8 * (lane + g);
   int slot_new = ring_base;
   for (int t = 0; t < ky; ++t) {
@@ -384,7 +414,7 @@ __device__ __forceinline__ void fast_pass_f(const uint16_t* __restrict__ ltile, 
     if (++slot_new == ring_slots) slot_new = 0;
   }
   int slot_old = ring_base;
-  for (int y = 0; y < F_RH; ++y) {
+  for (int y = 0; y < nrows; ++y) {
     if (y > 0) {
       {
         float Lv[8], Rv[16];
@@ -416,18 +446,17 @@ __device__ __forceinline__ void fast_pass_f(const uint16_t* __restrict__ ltile, 
 #pragma unroll
       for (int r = 0; r < 8; ++r) m[r] = (b == 0) ? o[r] : fminf(__fadd_rn(o[r], (float)b), m[r]);
     }
-    float* srow = state + y * F_COLS + lane;
+    unsigned long long* krow = keys + y * F_COLS + lane;      // high words: bits of the float cost*8 + 7
     float s8[8];
-    bool improved = false;
+    bool cand = false;
 #pragma unroll
-    for (int r = 0; r < 8; ++r) { s8[r] = srow[r * 32]; improved |= (m[r] < s8[r]); }
-    if (improved) {
+    for (int r = 0; r < 8; ++r) { s8[r] = __uint_as_float(key_hi(krow + r * 32)); cand |= (m[r] <= s8[r]); }
+    if (cand) {
 #pragma unroll
       for (int r = 0; r < 8; ++r) {
-        if (m[r] < s8[r]) {
+        if (m[r] <= s8[r]) {
           const int bi = (int)__float_as_uint(__fadd_rn(m[r], 8388608.0f)) & 7;
-          srow[r * 32] = __fsub_rn(m[r], (float)bi);
-          idxp[y * F_COLS + r * 32 + lane] = (uint16_t)(idx_base + bi);
+          offer_key(krow + r * 32, __float_as_uint(__fadd_rn(__fsub_rn(m[r], (float)bi), 7.0f)), (uint32_t)(idx_base + bi));
         }
       }
     }
@@ -437,17 +466,16 @@ __device__ __forceinline__ void fast_pass_f(const uint16_t* __restrict__ ltile, 
 template <int KX, bool FLT, bool FSEED, bool SQ = false>
 __global__ void __launch_bounds__(F_THREADS, 1)
 k1_fast_abs_kernel(const uint16_t* __restrict__ L16, const uint16_t* __restrict__ R16, FastGeom G,
-                   uint16_t* __restrict__ idx_scratch, vwb200_dispi* __restrict__ out, ptrdiff_t opitch,
-                   uint32_t* __restrict__ part_cost, uint16_t* __restrict__ part_idx) {
+                   vwb200_dispi* __restrict__ out, ptrdiff_t opitch, uint32_t* __restrict__ part_cost, uint16_t* __restrict__ part_idx) {
   extern __shared__ __align__(128) unsigned char smem[];
-  uint32_t* state = reinterpret_cast<uint32_t*>(smem);                                  // [4][32][8][32]
-  uint16_t* ltile = reinterpret_cast<uint16_t*>(smem + (size_t)F_SUBSETS * F_TH * F_COLS * 4);
+  unsigned long long* keys = reinterpret_cast<unsigned long long*>(smem);            // [th][8][32]: (cost << 32) | raster index
+  uint16_t* ltile = reinterpret_cast<uint16_t*>(smem + (size_t)G.th * F_COLS * 8);
   uint16_t* rring = ltile + (size_t)G.ltile_rows * F_COLS;
   uint64_t* bars = reinterpret_cast<uint64_t*>(rring + (size_t)G.ring_slots * G.rw);
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-  const int sub = w & (F_SUBSETS - 1), half = w / F_SUBSETS, row0 = half * F_RH;
   const int ngroups = (G.sx + F_B - 1) / F_B;
-  uint16_t* idxp_block = idx_scratch + (size_t)blockIdx.x * F_SUBSETS * F_TH * F_COLS;
+  // 1.7e38f as float bits / above every integer key / above every uint32 cost; low word above every raster index
+  const unsigned long long kinit = ((unsigned long long)(SQ ? 0xffffffffu : (FLT ? 0x7f000000u : FK_INIT_HI)) << 32) | 0xffffffffu;
   if (tid == 0) { mbar_init(&bars[0], 1); mbar_init(&bars[1], 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
   __syncthreads();
   uint32_t ph0 = 0, ph1 = 0;
@@ -455,7 +483,7 @@ k1_fast_abs_kernel(const uint16_t* __restrict__ L16, const uint16_t* __restrict_
   for (int item = blockIdx.x; item < G.NS * G.NB * G.J; item += gridDim.x) {
     const int chunk = item % G.J, rest = item / G.J;
     const int strip = rest % G.NS, band = rest / G.NS;
-    const int y0 = band * F_TH;
+    const int y0 = band * G.th, nrows = min(G.th, G.H - y0);
     const int dy0 = chunk * G.dy_per, ndy = min(G.sy, dy0 + G.dy_per) - dy0;
     const uint16_t* lsrc = L16 + ((size_t)strip * G.lrows + y0) * F_COLS;
     const uint16_t* rsrc = R16 + ((size_t)strip * G.rrows + y0 + dy0) * G.rw;
@@ -465,49 +493,39 @@ k1_fast_abs_kernel(const uint16_t* __restrict__ L16, const uint16_t* __restrict_
       tma_load_1d(ltile, lsrc, lbytes, &bars[0]);
       tma_load_1d(rring, rsrc, (uint32_t)G.ltile_rows * rrow_bytes, &bars[0]);     // right rows y0 .. y0+ltile_rows-1 -> slots 0..
     }
-    for (int k = tid; k < F_SUBSETS * F_TH * F_COLS; k += F_THREADS) state[k] = SQ ? 0xffffffffu : (FLT ? 0x7f000000u : S_INIT);     // 1.7e38f as float bits / max key
+    for (int k = tid; k < nrows * F_COLS; k += F_THREADS) keys[k] = kinit;
     __syncthreads();
     mbar_wait(&bars[0], ph0); ph0 ^= 1;
-    uint32_t* wstate = state + ((size_t)sub * F_TH + row0) * F_COLS;       // this warp's rows of its subset plane
-    uint16_t* widx = idxp_block + ((size_t)sub * F_TH + row0) * F_COLS;
     for (int dy = 0; dy < ndy; ++dy) {         // dy relative to the chunk's first row dy0
-      const int ring_base = (dy + row0) % G.ring_slots;
+      const int ring_base = dy % G.ring_slots;
       if (tid == 0 && dy + 1 < ndy) {        // prefetch the row iteration dy+1 adds, into the slot iteration dy-1 freed
         fence_proxy_async();
         mbar_expect_tx(&bars[1], rrow_bytes);
         tma_load_1d(rring + (size_t)((dy + G.ltile_rows) % G.ring_slots) * G.rw, rsrc + (size_t)(dy + G.ltile_rows) * G.rw, rrow_bytes, &bars[1]);
       }
-      for (int g = sub; g < ngroups; g += F_SUBSETS) {
-        if (SQ) fast_pass_sq<KX>(ltile, rring, wstate, widx, lane, g, G.ky, G.ring_slots, G.rw, ring_base, (dy0 + dy) * G.sx + F_B * g, row0,
-                                 min(F_B, G.sx - F_B * g));
-        else if (FLT) fast_pass_f<KX>(ltile, rring, reinterpret_cast<float*>(wstate), widx, lane, g, G.ky, G.ring_slots, G.rw, ring_base, (dy0 + dy) * G.sx + F_B * g, row0);
+      for (int g = w; g < ngroups; g += F_WARPS) {     // warp w: octets w, w+8, ... over all rows of the band
+        const int idx_base = (dy0 + dy) * G.sx + F_B * g;
+        if (SQ) fast_pass_sq<KX>(ltile, rring, keys, lane, g, G.ky, G.ring_slots, G.rw, ring_base, idx_base, nrows, min(F_B, G.sx - F_B * g));
+        else if (FLT) fast_pass_f<KX>(ltile, rring, keys, lane, g, G.ky, G.ring_slots, G.rw, ring_base, idx_base, nrows);
         else if (G.sx - F_B * g >= F_B)
-          fast_pass<KX, FSEED, true>(ltile, rring, wstate, widx, lane, g, G.ky, G.ring_slots, G.rw, ring_base, (dy0 + dy) * G.sx + F_B * g, row0, F_B);
+          fast_pass<KX, FSEED, true>(ltile, rring, keys, lane, g, G.ky, G.ring_slots, G.rw, ring_base, idx_base, nrows, F_B);
         else
-          fast_pass<KX, FSEED, false>(ltile, rring, wstate, widx, lane, g, G.ky, G.ring_slots, G.rw, ring_base, (dy0 + dy) * G.sx + F_B * g, row0,
-                                      G.sx - F_B * g);
+          fast_pass<KX, FSEED, false>(ltile, rring, keys, lane, g, G.ky, G.ring_slots, G.rw, ring_base, idx_base, nrows, G.sx - F_B * g);
       }
       if (dy + 1 < ndy) { mbar_wait(&bars[1], ph1); ph1 ^= 1; }
       __syncthreads();
     }
-    // ---- merge the 4 warps' private bests and write {dx, dy, valid} ----
-    const int nw = ngroups < F_SUBSETS ? ngroups : F_SUBSETS;
+    // ---- write {dx, dy, valid} (or this dy chunk's partial result) ----
     const int s0 = strip * G.out_cols;
-    for (int pix = tid; pix < F_TH * G.out_cols; pix += F_THREADS) {
+    for (int pix = tid; pix < nrows * G.out_cols; pix += F_THREADS) {
       const int x = pix % G.out_cols, y = pix / G.out_cols;
       const int gx = s0 + x, gy = y0 + y;
-      if (gx >= G.W || gy >= G.H) continue;
-      const int off = y * F_COLS + (x & 7) * 32 + (x >> 3);
-      uint32_t best = state[off];
-      int bidx = idxp_block[off];
-      for (int ww = 1; ww < nw; ++ww) {
-        const uint32_t c = state[(size_t)ww * F_TH * F_COLS + off];
-        const int i = idxp_block[(size_t)ww * F_TH * F_COLS + off];
-        if (c < best || (c == best && i < bidx)) { best = c; bidx = i; }
-      }
+      if (gx >= G.W) continue;
+      const unsigned long long key = keys[y * F_COLS + (x & 7) * 32 + (x >> 3)];
+      const int bidx = (int)(uint32_t)key;
       if (G.J > 1) {             // partial result of this dy chunk; k1_fast_merge_kernel finishes the pixel
         const size_t pk = ((size_t)chunk * G.H + gy) * G.W + gx;
-        part_cost[pk] = best; part_idx[pk] = (uint16_t)bidx;
+        part_cost[pk] = (uint32_t)(key >> 32); part_idx[pk] = (uint16_t)bidx;
         continue;
       }
       vwb200_dispi o;
@@ -564,7 +582,7 @@ int k1_fast_launch(int cost, ImgF left, ImgF right, int W, int H, int sx, int sy
                    const KEvents* ev, const FastOrigin* org) {
   (void)workspace_bytes;
   const bool sq = cost == VWB200_SQUARED_DIFFERENCE;
-  FastGeom g = make_geom(W, H, sx, sy, kx, ky);
+  FastGeom g = fast_geom(W, H, sx, sy, kx, ky);
   g.scale = sq ? 1 : F_B;
   if (org) { g.lox = org->lox; g.loy = org->loy; g.rox = org->rox; g.roy = org->roy; g.addx = org->addx; g.addy = org->addy; }
   // fp32 carries the integers exactly while every window sum * 8 (+7) stays below 2^24
@@ -578,8 +596,7 @@ int k1_fast_launch(int cost, ImgF left, ImgF right, int W, int H, int sx, int sy
   unsigned char* ws = static_cast<unsigned char*>(workspace);
   uint16_t* L16 = reinterpret_cast<uint16_t*>(ws);
   uint16_t* R16 = L16 + (size_t)g.NS * g.lrows * F_COLS;
-  uint16_t* idx = R16 + (size_t)g.NS * g.rrows * g.rw;
-  uint32_t* part_cost = reinterpret_cast<uint32_t*>(reinterpret_cast<uintptr_t>(idx + (size_t)1024 * F_SUBSETS * F_TH * F_COLS + 31) & ~(uintptr_t)63);
+  uint32_t* part_cost = reinterpret_cast<uint32_t*>((reinterpret_cast<uintptr_t>(R16 + (size_t)g.NS * g.rrows * g.rw) + 63) & ~(uintptr_t)63);
   uint16_t* part_idx = reinterpret_cast<uint16_t*>(part_cost + (size_t)g.J * W * H);
   {
     dim3 gl(g.lrows, g.NS), gr(g.rrows, g.NS);
@@ -594,7 +611,7 @@ int k1_fast_launch(int cost, ImgF left, ImgF right, int W, int H, int sx, int sy
   const int items = g.NS * g.NB * g.J;
   const int grid = items < nsm ? items : nsm;
   const size_t smem = fast_smem_bytes(g);
-  void (*kern)(const uint16_t*, const uint16_t*, FastGeom, uint16_t*, vwb200_dispi*, ptrdiff_t, uint32_t*, uint16_t*) = nullptr;
+  void (*kern)(const uint16_t*, const uint16_t*, FastGeom, vwb200_dispi*, ptrdiff_t, uint32_t*, uint16_t*) = nullptr;
   switch (kx) {
 #define KCASE(K) case K: kern = sq ? k1_fast_abs_kernel<K, false, false, true> : (use_float ? k1_fast_abs_kernel<K, true, false> : (float_seed ? k1_fast_abs_kernel<K, false, true> : k1_fast_abs_kernel<K, false, false>)); break;
     KCASE(3) KCASE(5) KCASE(7) KCASE(9) KCASE(11) KCASE(13) KCASE(15) KCASE(17) KCASE(19) KCASE(21) KCASE(23) KCASE(25)
@@ -602,9 +619,9 @@ int k1_fast_launch(int cost, ImgF left, ImgF right, int W, int H, int sx, int sy
 #undef KCASE
     default: set_error("k1_fast: unsupported kernel width %d", kx); return VWB200_ENOIMPL;
   }
-  VWB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));   // per-function state shared by all host threads: device maximum
+  VWB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FK_SMEM));   // per-function state shared by all host threads: device maximum
   if (ev && ev->e0) cudaEventRecord(ev->e0, st);
-  kern<<<grid, F_THREADS, smem, st>>>(L16, R16, g, idx, out, opitch, part_cost, part_idx);
+  kern<<<grid, F_THREADS, smem, st>>>(L16, R16, g, out, opitch, part_cost, part_idx);
   VWB_LAUNCH_CHECK();
   if (ev && ev->e1) cudaEventRecord(ev->e1, st);
   if (g.J > 1) {

@@ -5,15 +5,14 @@
 
 namespace vwb200 {
 
-static constexpr int F_TH = 32;        // output rows per band
+static constexpr int F_TH = 32;        // output rows per band of k1_screen (k1_fast: FastGeom::th)
 static constexpr int F_COLS = 256;     // padded columns per strip (32 lanes x 8)
-static constexpr int F_WARPS = 8;       // 4 dx subsets x 2 row halves (2 warps per SM sub-partition)
+static constexpr int F_WARPS = 8;       // per CTA (2 per SM sub-partition); k1_screen: 4 dx subsets x 2 row halves
 static constexpr int F_SUBSETS = 4;
 static constexpr int F_HALVES = F_WARPS / F_SUBSETS;
 static constexpr int F_RH = F_TH / F_HALVES;      // output rows per warp
 static constexpr int F_THREADS = F_WARPS * 32;
 static constexpr int F_B = 8;          // consecutive dx per thread (one "octet"); keys are cost*8 + b
-static constexpr uint32_t S_INIT = 0x7ffffff8u;
 
 // ---- geometry -----------------------------------------------------------------------------------------
 struct FastGeom {
@@ -21,8 +20,8 @@ struct FastGeom {
   int out_cols;      // output columns per strip = 256 - (kx-1)
   int NS, NB;        // strips, bands
   int lrows, rrows;  // padded row counts of the packed arrays
-  int ltile_rows;    // F_TH + ky - 1
-  int ring_slots;    // F_TH + ky
+  int ltile_rows;    // th + ky - 1
+  int ring_slots;    // th + ky
   int rw;            // u16 per packed right row = 256 + sx (multiple of 8)
   int scale;                // values are packed as (v - vmin) * scale: 8 for AbsoluteCost (keys = cost*8+b), 1 for SquaredCost
   int J, dy_per;            // the dy range is split into J chunks of dy_per rows (more, smaller work items for small rasters)
@@ -30,17 +29,18 @@ struct FastGeom {
   int addx, addy;           // constant added to the output disparities
   int sd;                   // k1_screen: dy rows per synchronisation period (ring depth)
   int dynamic_units;          // k1_screen: 1 = warps draw (octet, half) work units from a shared counter, 0 = static round-robin
+  int th;                   // output rows per band (F_TH for k1_screen; k1_fast sizes it from its shared-memory budget)
 };
-static inline FastGeom make_geom(int W, int H, int sx, int sy, int kx, int ky) {
+static inline FastGeom make_geom(int W, int H, int sx, int sy, int kx, int ky, int th = F_TH) {
   FastGeom g;
-  g.W = W; g.H = H; g.sx = sx; g.sy = sy; g.kx = kx; g.ky = ky;
+  g.W = W; g.H = H; g.sx = sx; g.sy = sy; g.kx = kx; g.ky = ky; g.th = th;
   g.out_cols = F_COLS - (kx - 1);
   g.NS = (W + g.out_cols - 1) / g.out_cols;
-  g.NB = (H + F_TH - 1) / F_TH;
-  g.ltile_rows = F_TH + ky - 1;
-  g.ring_slots = F_TH + ky;
-  g.lrows = g.NB * F_TH + ky - 1;
-  g.rrows = g.NB * F_TH + ky - 1 + sy;
+  g.NB = (H + th - 1) / th;
+  g.ltile_rows = th + ky - 1;
+  g.ring_slots = th + ky;
+  g.lrows = g.NB * th + ky - 1;
+  g.rrows = g.NB * th + ky - 1 + sy;
   g.rw = ((F_COLS + sx + 7) / 8) * 8 + 8;
   g.lox = g.loy = g.rox = g.roy = 0; g.addx = g.addy = 0; g.scale = F_B; g.dynamic_units = 1; g.sd = 1;
   // The work items (strip x band x dy-chunk) are dealt round-robin to kNumSMs persistent CTAs, so the last partial wave idles
@@ -65,10 +65,6 @@ static inline FastGeom make_geom(int W, int H, int sx, int sy, int kx, int ky) {
   g.J = (sy + g.dy_per - 1) / g.dy_per;
   return g;
 }
-static inline size_t fast_smem_bytes(const FastGeom& g) {
-  return (size_t)F_SUBSETS * F_TH * F_COLS * 4 + (size_t)g.ltile_rows * F_COLS * 2 + (size_t)g.ring_slots * g.rw * 2 + 64;
-}
-
 // ---- PTX helpers: mbarrier + TMA bulk copy -----------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
