@@ -2,6 +2,7 @@
 // from, measured on an H100 (sm_90a).  Output feeds DESIGN.md's ALU/MIO roofline for K1.
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o microbench microbench.cu
 #include <cstdio>
+#include <cstdlib>
 #include <cuda_runtime.h>
 
 #define ITERS 4096
@@ -37,6 +38,8 @@ __global__ void __launch_bounds__(1024) bench(float* out, int seed, long long* c
       if (OP == 13) { int t = __vabsdiffs2(v[k], ia); v[k] += t; }
       if (OP == 14) v[k] = abs(v[k] - ia) + it;                           // IABS path
       if (OP == 15) { asm volatile("{.reg .pred p; setp.lt.s32 p, %1, %0; @p mov.s32 %0, %1;}" : "+r"(v[k]) : "r"(ia ^ it)); }
+      if (OP == 16) { if (k & 1) f[k] = __fadd_rn(f[k], fa); else v[k] = __sad(v[k], ia, v[k]); }   // ALU and FMA pipes side by side
+      if (OP == 17) v[k] = min(v[k] + ia, it);                                                       // VIADDMNMX
     }
   }
   long long t1 = clock64();
@@ -68,12 +71,15 @@ void run(const char* name, int threads, int blocks_per_sm, int nsm) {
   cudaFree(out); cudaFree(cyc);
 }
 
-int main() {
+// Usage: microbench [threads per SM ...]   (default: 128 256 1024; K1 fast runs 256 = 8 warps per SM)
+int main(int argc, char** argv) {
   cudaDeviceProp p; cudaGetDeviceProperties(&p, 0);
   printf("%s  SMs=%d  clock=%d kHz\n", p.name, p.multiProcessorCount, p.clockRate);
   int nsm = p.multiProcessorCount;
-  for (int cfg = 0; cfg < 2; ++cfg) {
-    int threads = cfg == 0 ? 128 : 1024, bps = 1;
+  int cfgs[16] = {128, 256, 1024}, ncfg = 3;
+  if (argc > 1) { ncfg = 0; for (int i = 1; i < argc && ncfg < 16; ++i) cfgs[ncfg++] = atoi(argv[i]); }
+  for (int cfg = 0; cfg < ncfg; ++cfg) {
+    int threads = cfgs[cfg], bps = 1;
     printf("---- %d threads per SM ----\n", threads);
     run<0>("FADD", threads, bps, nsm);
     run<1>("FFMA", threads, bps, nsm);
@@ -91,6 +97,8 @@ int main() {
     run<13>("VABSDIFF2+IADD", threads, bps, nsm);
     run<14>("IABS(a-b)+c", threads, bps, nsm);
     run<15>("SETP+predMOV", threads, bps, nsm);
+    run<16>("SAD|FADD 1:1", threads, bps, nsm);
+    run<17>("VIADDMNMX", threads, bps, nsm);
   }
   return 0;
 }

@@ -8,7 +8,7 @@
 // reference while doing ~10 issue slots per (pixel, disparity) instead of ~70 bytes of DRAM traffic.
 //
 // Decomposition (persistent CTAs of 8 warps, one CTA per SM; work item = 236-column x th-row band, th chosen by
-// fast_geom within the shared-memory budget -- up to 61 rows at 128 x 128 / 21 x 21):
+// fast_geom within the shared-memory budget -- 84 rows at 128 x 128 / 21 x 21):
 //   * values are pre-packed (pack kernels) as u16 (v-vmin)*8, one contiguous row per strip, so that a
 //     lane fetches its 8 left / 16 right columns with conflict-free 16-byte LDS.128 loads
 //   * the left tile (th+ky-1 rows) and a ring of right rows are staged in shared memory with TMA bulk
@@ -20,15 +20,14 @@
 //   * the kx-wide horizontal sums are formed without shared memory: in-lane prefix sums + 9 warp
 //     shuffles per 8 outputs (blocked-prefix scheme), 3-input IADD3
 //   * arg-best: costs are pre-scaled by 8 so key = cost*8 + b; min over the 8 dx is 7 VIADDMNMX;
-//     one shared-memory plane holds a 64-bit key (cost << 32 | raster index) per band pixel.  The hot
-//     loop reads only the high words; the (rare) candidates with a cost <= the stored one go through a
-//     64-bit atomicMin, so the lowest cost and, among equal costs, the first disparity in raster order
-//     wins whichever warp reaches it first
+//     a shared-memory plane holds the best high word (cost*8 | 7) per band pixel, the threshold of the hot loop;
+//     the (rare) candidates with a cost <= it lower it with a 32-bit atomicMin and send the exact 64-bit key
+//     (cost << 32 | raster index) to a per-CTA plane in global memory with a 64-bit atomicMin reduction -- neither
+//     is waited for -- so the lowest cost and, among equal costs, the first disparity in raster order wins
+//     whichever warp reaches it first
 //   * pixels whose arg-best is disparity (0,0) are re-checked by a small kernel for the
 //     "every disparity gave the same cost => invalid" rule (Correlation.cc:121-133)
 #include "k1_fast_common.cuh"
-#include <cstdlib>
-#include <cstring>
 
 namespace vwb200 {
 
@@ -75,13 +74,13 @@ int image_stats_launch(ImgF img, float* d_result3, cudaStream_t st) {
 }
 
 // ---- band geometry ------------------------------------------------------------------------------------------------
-static constexpr int FK_TH_MAX = 64;                 // tallest band considered (the headline fits 61 rows)
+static constexpr int FK_TH_MAX = 96;                 // tallest band considered
 static constexpr size_t FK_SMEM = 227 * 1024;
 static constexpr uint32_t FK_INIT_HI = 0x7fffffffu;  // high word of an empty key: above every (cost*8 | 7)
 
-// key plane [th][256] (u64) | left tile [th+ky-1][256] (u16) | right ring [th+ky][rw] (u16) | 2 mbarriers
+// best plane [th][256] (u32) | left tile [th+ky-1][256] (u16) | right ring [th+ky][rw] (u16) | 2 mbarriers
 static size_t fast_smem_bytes(const FastGeom& g) {
-  return (size_t)g.th * F_COLS * 8 + (size_t)g.ltile_rows * F_COLS * 2 + (size_t)g.ring_slots * g.rw * 2 + 64;
+  return (size_t)g.th * F_COLS * 4 + (size_t)g.ltile_rows * F_COLS * 2 + (size_t)g.ring_slots * g.rw * 2 + 64;
 }
 
 // Band height: a taller band spreads the seeding of each (dy, octet) -- ky rows of vertical sums plus a first row
@@ -124,7 +123,8 @@ size_t k1_fast_workspace_bytes(int W, int H, int sx, int sy, int kx, int ky) {
   size_t l = (size_t)g.NS * g.lrows * F_COLS * 2;
   size_t r = (size_t)g.NS * g.rrows * g.rw * 2;
   size_t part = g.J > 1 ? (size_t)g.J * W * H * 6 + 64 : 0;      // per-dy-chunk partial (cost u32, index u16)
-  return l + r + part + 512;
+  size_t keys = (size_t)kNumSMs * g.th * F_COLS * 8 + 64;           // one 64-bit key plane per persistent CTA
+  return l + r + part + keys + 512;
 }
 
 // ---- pack kernels: float raster -> u16 (v - vmin) * 4 in the lane-transposed strip layout ------------
@@ -173,72 +173,36 @@ __device__ __forceinline__ void load_row(const uint16_t* lrow, const uint16_t* r
   for (int i = 0; i < 8; ++i) Rv[8 + i] = t[i];
 }
 
-__device__ __forceinline__ void unpack8f(const uint4 v, float (&o)[8]) {
-  o[0] = __uint_as_float(__byte_perm(v.x, 0x4B000000u, 0x7610)); o[1] = __uint_as_float(__byte_perm(v.x, 0x4B000000u, 0x7632));
-  o[2] = __uint_as_float(__byte_perm(v.y, 0x4B000000u, 0x7610)); o[3] = __uint_as_float(__byte_perm(v.y, 0x4B000000u, 0x7632));
-  o[4] = __uint_as_float(__byte_perm(v.z, 0x4B000000u, 0x7610)); o[5] = __uint_as_float(__byte_perm(v.z, 0x4B000000u, 0x7632));
-  o[6] = __uint_as_float(__byte_perm(v.w, 0x4B000000u, 0x7610)); o[7] = __uint_as_float(__byte_perm(v.w, 0x4B000000u, 0x7632));
-}
-__device__ __forceinline__ void load_row_f(const uint16_t* lrow, const uint16_t* rrow, float (&Lv)[8], float (&Rv)[16]) {
-  unpack8f(*reinterpret_cast<const uint4*>(lrow), Lv);
-  float t[8];
-  unpack8f(*reinterpret_cast<const uint4*>(rrow), t);
-#pragma unroll
-  for (int i = 0; i < 8; ++i) Rv[i] = t[i];
-  unpack8f(*reinterpret_cast<const uint4*>(rrow + 8), t);
-#pragma unroll
-  for (int i = 0; i < 8; ++i) Rv[8 + i] = t[i];
-}
-// High word of a pixel's key in the shared plane (the hot loop compares costs only).
-__device__ __forceinline__ uint32_t key_hi(const unsigned long long* k) { return reinterpret_cast<const uint32_t*>(k)[1]; }
-// A candidate: keep the lower cost and, for equal costs, the lower raster index (= the first disparity).
-__device__ __forceinline__ void offer_key(unsigned long long* k, uint32_t hi, uint32_t idx) {
-  atomicMin(k, ((unsigned long long)hi << 32) | idx);
+// A candidate: keep the lower cost and, for equal costs, the lower raster index (= the first disparity).  The exact
+// 64-bit key (hi << 32 | raster index) goes to the CTA's plane in global memory, where a 64-bit atomicMin is one
+// native reduction; the shared plane keeps only the high word, the threshold the hot loop compares with (a native
+// 32-bit shared atomicMin).  Neither result is waited for.  A stale threshold only lets more candidates through.
+__device__ __forceinline__ void offer_key(uint32_t* best, unsigned long long* key, uint32_t hi, uint32_t idx) {
+  atomicMin(best, hi);
+  atomicMin(key, ((unsigned long long)hi << 32) | idx);
 }
 
-template <int KX, bool FSEED, bool FULL>
+template <int KX, bool FULL>
 __device__ __forceinline__ void fast_pass(const uint16_t* __restrict__ ltile, const uint16_t* __restrict__ rring,
-                                          unsigned long long* __restrict__ keys,
+                                          uint32_t* __restrict__ best, unsigned long long* __restrict__ keys,
                                           int lane, int g, int ky, int ring_slots, int rw, int ring_base, int idx_base, int nrows, int nb) {
   int V[8][F_B];
   const uint16_t* lp = ltile + 8 * lane;                       // + row*256            (16-byte aligned)
   const uint16_t* rp = rring + 8 * (lane + g);                 // + slot*rw            (16-byte aligned)
   int slot_new = ring_base;                                     // ring slot of right row (dy + t)
-  // ---- seed: first ky rows.  The integer main loop is bound by the ALU pipe (VABSDIFF), so the seed
-  //      rows are summed in fp32 on the otherwise idle FMA pipes (exact: sums < 2^23) and converted once.
-  if (FSEED) {
-    float Vf[8][F_B];
+  // ---- seed: first ky rows ----
+#pragma unroll
+  for (int a = 0; a < 8; ++a)
+#pragma unroll
+    for (int b = 0; b < F_B; ++b) V[a][b] = 0;
+  for (int t = 0; t < ky; ++t) {
+    int Lv[8], Rv[16];
+    load_row(lp + t * F_COLS, rp + slot_new * rw, Lv, Rv);
 #pragma unroll
     for (int a = 0; a < 8; ++a)
 #pragma unroll
-      for (int b = 0; b < F_B; ++b) Vf[a][b] = 0.0f;
-    for (int t = 0; t < ky; ++t) {
-      float Lv[8], Rv[16];
-      load_row_f(lp + t * F_COLS, rp + slot_new * rw, Lv, Rv);
-#pragma unroll
-      for (int a = 0; a < 8; ++a)
-#pragma unroll
-        for (int b = 0; b < F_B; ++b) Vf[a][b] = __fadd_rn(Vf[a][b], fabsf(__fsub_rn(Lv[a], Rv[a + b])));
-      if (++slot_new == ring_slots) slot_new = 0;
-    }
-#pragma unroll
-    for (int a = 0; a < 8; ++a)
-#pragma unroll
-      for (int b = 0; b < F_B; ++b) V[a][b] = (int)__float_as_uint(__fadd_rn(Vf[a][b], 8388608.0f)) - 0x4B000000;
-  } else {
-#pragma unroll
-    for (int a = 0; a < 8; ++a)
-#pragma unroll
-      for (int b = 0; b < F_B; ++b) V[a][b] = 0;
-    for (int t = 0; t < ky; ++t) {
-      int Lv[8], Rv[16];
-      load_row(lp + t * F_COLS, rp + slot_new * rw, Lv, Rv);
-#pragma unroll
-      for (int a = 0; a < 8; ++a)
-#pragma unroll
-        for (int b = 0; b < F_B; ++b) V[a][b] = __sad(Lv[a], Rv[a + b], V[a][b]);
-      if (++slot_new == ring_slots) slot_new = 0;
-    }
+      for (int b = 0; b < F_B; ++b) V[a][b] = __sad(Lv[a], Rv[a + b], V[a][b]);
+    if (++slot_new == ring_slots) slot_new = 0;
   }
   int slot_old = ring_base;
   for (int y = 0; y < nrows; ++y) {
@@ -277,15 +241,16 @@ __device__ __forceinline__ void fast_pass(const uint16_t* __restrict__ ltile, co
     }
     // ---- running best: high words hold cost*8 | 7, so m <= s <=> cost <= best cost.  Equal costs are candidates
     //      too: another warp may hold the same cost at a later disparity ----
+    uint32_t* brow = best + y * F_COLS + lane;
     unsigned long long* krow = keys + y * F_COLS + lane;
     uint32_t s8[8];
     bool cand = false;
 #pragma unroll
-    for (int r = 0; r < 8; ++r) { s8[r] = key_hi(krow + r * 32); cand |= ((uint32_t)m[r] <= s8[r]); }
+    for (int r = 0; r < 8; ++r) { s8[r] = brow[r * 32]; cand |= ((uint32_t)m[r] <= s8[r]); }
     if (cand) {                // rare once the search has seen the neighbourhood of the true match
 #pragma unroll
       for (int r = 0; r < 8; ++r)
-        if ((uint32_t)m[r] <= s8[r]) offer_key(krow + r * 32, (uint32_t)m[r] | 7u, (uint32_t)(idx_base + (m[r] & 7)));
+        if ((uint32_t)m[r] <= s8[r]) offer_key(brow + r * 32, krow + r * 32, (uint32_t)m[r] | 7u, (uint32_t)(idx_base + (m[r] & 7)));
     }
   }
 }
@@ -296,7 +261,7 @@ __device__ __forceinline__ void fast_pass(const uint16_t* __restrict__ ltile, co
 // leave room for the key trick, so the arg-min over the octet is tracked with compare/select.
 template <int KX>
 __device__ __forceinline__ void fast_pass_sq(const uint16_t* __restrict__ ltile, const uint16_t* __restrict__ rring,
-                                             unsigned long long* __restrict__ keys,
+                                             uint32_t* __restrict__ best, unsigned long long* __restrict__ keys,
                                              int lane, int g, int ky, int ring_slots, int rw, int ring_base, int idx_base, int nrows, int nb) {
   int V[8][F_B];
 #pragma unroll
@@ -354,128 +319,29 @@ __device__ __forceinline__ void fast_pass_sq(const uint16_t* __restrict__ ltile,
         else if (c < m[r]) { m[r] = c; mb[r] = b; }
       }
     }
-    unsigned long long* krow = keys + y * F_COLS + lane;      // high words: the uint32 cost
+    uint32_t* brow = best + y * F_COLS + lane;                 // high words: the uint32 cost
+    unsigned long long* krow = keys + y * F_COLS + lane;
 #pragma unroll
     for (int r = 0; r < 8; ++r)
-      if (m[r] <= key_hi(krow + r * 32)) offer_key(krow + r * 32, m[r], (uint32_t)(idx_base + mb[r]));
+      if (m[r] <= brow[r * 32]) offer_key(brow + r * 32, krow + r * 32, m[r], (uint32_t)(idx_base + mb[r]));
   }
 }
 
-// ---- float variant of the pass: the same exact integers carried in fp32 ----------------------------------
-// The ALU pipe (VABSDIFF, integer min, unpack) is the bound of the integer pass; FADD runs on the FMA
-// pipes at twice the ALU rate.  Unpacking u16 -> "2^23 + x" biased floats is a single PRMT, differences
-// of biased floats are exact, and every sum stays below 2^24 (checked on the host), so the fp32 pass
-// produces the same integers.
-template <int KX>
-__device__ __forceinline__ void window_sums_f(const float (&p)[8], float (&out)[8]) {
-  const float T = p[7];
-  constexpr int MAXL = (KX - 1) / 8;
-  float W[MAXL + 1];
-  W[0] = T;
-#pragma unroll
-  for (int k = 1; k <= MAXL; ++k) W[k] = __fadd_rn(W[k - 1], __shfl_down_sync(0xffffffffu, T, k));
-#pragma unroll
-  for (int r = 0; r < 8; ++r) {
-    const int own = 8 - r;
-    if (KX <= own) {
-      out[r] = r ? __fsub_rn(p[r + KX - 1], p[r - 1]) : p[KX - 1];
-    } else {
-      const int rem = KX - own;
-      const int full = rem / 8, part = rem % 8;
-      if (part) {
-        const float q = __shfl_down_sync(0xffffffffu, p[part - 1], full + 1);
-        out[r] = r ? __fadd_rn(__fsub_rn(W[full], p[r - 1]), q) : __fadd_rn(W[full], q);
-      } else {
-        out[r] = r ? __fsub_rn(W[full], p[r - 1]) : W[full];
-      }
-    }
-  }
-}
-
-template <int KX>
-__device__ __forceinline__ void fast_pass_f(const uint16_t* __restrict__ ltile, const uint16_t* __restrict__ rring,
-                                            unsigned long long* __restrict__ keys,
-                                            int lane, int g, int ky, int ring_slots, int rw, int ring_base, int idx_base, int nrows) {
-  float V[8][F_B];
-#pragma unroll
-  for (int a = 0; a < 8; ++a)
-#pragma unroll
-    for (int b = 0; b < F_B; ++b) V[a][b] = 0.0f;
-  const uint16_t* lp = ltile + 8 * lane;
-  const uint16_t* rp = rring + 8 * (lane + g);
-  int slot_new = ring_base;
-  for (int t = 0; t < ky; ++t) {
-    float Lv[8], Rv[16];
-    load_row_f(lp + t * F_COLS, rp + slot_new * rw, Lv, Rv);
-#pragma unroll
-    for (int a = 0; a < 8; ++a)
-#pragma unroll
-      for (int b = 0; b < F_B; ++b) V[a][b] = __fadd_rn(V[a][b], fabsf(__fsub_rn(Lv[a], Rv[a + b])));
-    if (++slot_new == ring_slots) slot_new = 0;
-  }
-  int slot_old = ring_base;
-  for (int y = 0; y < nrows; ++y) {
-    if (y > 0) {
-      {
-        float Lv[8], Rv[16];
-        load_row_f(lp + (y + ky - 1) * F_COLS, rp + slot_new * rw, Lv, Rv);
-#pragma unroll
-        for (int a = 0; a < 8; ++a)
-#pragma unroll
-          for (int b = 0; b < F_B; ++b) V[a][b] = __fadd_rn(V[a][b], fabsf(__fsub_rn(Lv[a], Rv[a + b])));
-      }
-      {
-        float Lo[8], Ro[16];
-        load_row_f(lp + (y - 1) * F_COLS, rp + slot_old * rw, Lo, Ro);
-#pragma unroll
-        for (int a = 0; a < 8; ++a)
-#pragma unroll
-          for (int b = 0; b < F_B; ++b) V[a][b] = __fsub_rn(V[a][b], fabsf(__fsub_rn(Lo[a], Ro[a + b])));
-      }
-      if (++slot_new == ring_slots) slot_new = 0;
-      if (++slot_old == ring_slots) slot_old = 0;
-    }
-    float m[8];
-#pragma unroll
-    for (int b = 0; b < F_B; ++b) {
-      float p[8], o[8];
-      p[0] = V[0][b];
-#pragma unroll
-      for (int a = 1; a < 8; ++a) p[a] = __fadd_rn(p[a - 1], V[a][b]);
-      window_sums_f<KX>(p, o);
-#pragma unroll
-      for (int r = 0; r < 8; ++r) m[r] = (b == 0) ? o[r] : fminf(__fadd_rn(o[r], (float)b), m[r]);
-    }
-    unsigned long long* krow = keys + y * F_COLS + lane;      // high words: bits of the float cost*8 + 7
-    float s8[8];
-    bool cand = false;
-#pragma unroll
-    for (int r = 0; r < 8; ++r) { s8[r] = __uint_as_float(key_hi(krow + r * 32)); cand |= (m[r] <= s8[r]); }
-    if (cand) {
-#pragma unroll
-      for (int r = 0; r < 8; ++r) {
-        if (m[r] <= s8[r]) {
-          const int bi = (int)__float_as_uint(__fadd_rn(m[r], 8388608.0f)) & 7;
-          offer_key(krow + r * 32, __float_as_uint(__fadd_rn(__fsub_rn(m[r], (float)bi), 7.0f)), (uint32_t)(idx_base + bi));
-        }
-      }
-    }
-  }
-}
-
-template <int KX, bool FLT, bool FSEED, bool SQ = false>
+template <int KX, bool SQ = false>
 __global__ void __launch_bounds__(F_THREADS, 1)
 k1_fast_abs_kernel(const uint16_t* __restrict__ L16, const uint16_t* __restrict__ R16, FastGeom G,
-                   vwb200_dispi* __restrict__ out, ptrdiff_t opitch, uint32_t* __restrict__ part_cost, uint16_t* __restrict__ part_idx) {
+                   vwb200_dispi* __restrict__ out, ptrdiff_t opitch, uint32_t* __restrict__ part_cost, uint16_t* __restrict__ part_idx,
+                   unsigned long long* __restrict__ gkeys) {
   extern __shared__ __align__(128) unsigned char smem[];
-  unsigned long long* keys = reinterpret_cast<unsigned long long*>(smem);            // [th][8][32]: (cost << 32) | raster index
-  uint16_t* ltile = reinterpret_cast<uint16_t*>(smem + (size_t)G.th * F_COLS * 8);
+  uint32_t* best = reinterpret_cast<uint32_t*>(smem);                                  // [th][8][32]: best high word
+  unsigned long long* keys = gkeys + (size_t)blockIdx.x * G.th * F_COLS;               // [th][8][32]: (high word << 32) | raster index
+  uint16_t* ltile = reinterpret_cast<uint16_t*>(smem + (size_t)G.th * F_COLS * 4);
   uint16_t* rring = ltile + (size_t)G.ltile_rows * F_COLS;
   uint64_t* bars = reinterpret_cast<uint64_t*>(rring + (size_t)G.ring_slots * G.rw);
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   const int ngroups = (G.sx + F_B - 1) / F_B;
-  // 1.7e38f as float bits / above every integer key / above every uint32 cost; low word above every raster index
-  const unsigned long long kinit = ((unsigned long long)(SQ ? 0xffffffffu : (FLT ? 0x7f000000u : FK_INIT_HI)) << 32) | 0xffffffffu;
+  // above every integer key / above every uint32 cost; low word above every raster index
+  const unsigned long long kinit = ((unsigned long long)(SQ ? 0xffffffffu : FK_INIT_HI) << 32) | 0xffffffffu;
   if (tid == 0) { mbar_init(&bars[0], 1); mbar_init(&bars[1], 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
   __syncthreads();
   uint32_t ph0 = 0, ph1 = 0;
@@ -493,7 +359,7 @@ k1_fast_abs_kernel(const uint16_t* __restrict__ L16, const uint16_t* __restrict_
       tma_load_1d(ltile, lsrc, lbytes, &bars[0]);
       tma_load_1d(rring, rsrc, (uint32_t)G.ltile_rows * rrow_bytes, &bars[0]);     // right rows y0 .. y0+ltile_rows-1 -> slots 0..
     }
-    for (int k = tid; k < nrows * F_COLS; k += F_THREADS) keys[k] = kinit;
+    for (int k = tid; k < nrows * F_COLS; k += F_THREADS) { best[k] = (uint32_t)(kinit >> 32); keys[k] = kinit; }
     __syncthreads();
     mbar_wait(&bars[0], ph0); ph0 ^= 1;
     for (int dy = 0; dy < ndy; ++dy) {         // dy relative to the chunk's first row dy0
@@ -505,12 +371,11 @@ k1_fast_abs_kernel(const uint16_t* __restrict__ L16, const uint16_t* __restrict_
       }
       for (int g = w; g < ngroups; g += F_WARPS) {     // warp w: octets w, w+8, ... over all rows of the band
         const int idx_base = (dy0 + dy) * G.sx + F_B * g;
-        if (SQ) fast_pass_sq<KX>(ltile, rring, keys, lane, g, G.ky, G.ring_slots, G.rw, ring_base, idx_base, nrows, min(F_B, G.sx - F_B * g));
-        else if (FLT) fast_pass_f<KX>(ltile, rring, keys, lane, g, G.ky, G.ring_slots, G.rw, ring_base, idx_base, nrows);
+        if (SQ) fast_pass_sq<KX>(ltile, rring, best, keys, lane, g, G.ky, G.ring_slots, G.rw, ring_base, idx_base, nrows, min(F_B, G.sx - F_B * g));
         else if (G.sx - F_B * g >= F_B)
-          fast_pass<KX, FSEED, true>(ltile, rring, keys, lane, g, G.ky, G.ring_slots, G.rw, ring_base, idx_base, nrows, F_B);
+          fast_pass<KX, true>(ltile, rring, best, keys, lane, g, G.ky, G.ring_slots, G.rw, ring_base, idx_base, nrows, F_B);
         else
-          fast_pass<KX, FSEED, false>(ltile, rring, keys, lane, g, G.ky, G.ring_slots, G.rw, ring_base, idx_base, nrows, G.sx - F_B * g);
+          fast_pass<KX, false>(ltile, rring, best, keys, lane, g, G.ky, G.ring_slots, G.rw, ring_base, idx_base, nrows, G.sx - F_B * g);
       }
       if (dy + 1 < ndy) { mbar_wait(&bars[1], ph1); ph1 ^= 1; }
       __syncthreads();
@@ -521,7 +386,8 @@ k1_fast_abs_kernel(const uint16_t* __restrict__ L16, const uint16_t* __restrict_
       const int x = pix % G.out_cols, y = pix / G.out_cols;
       const int gx = s0 + x, gy = y0 + y;
       if (gx >= G.W) continue;
-      const unsigned long long key = keys[y * F_COLS + (x & 7) * 32 + (x >> 3)];
+      // the reductions were performed in L2 after the barrier that ended the dy loop: read past L1
+      const unsigned long long key = __ldcg(keys + y * F_COLS + (x & 7) * 32 + (x >> 3));
       const int bidx = (int)(uint32_t)key;
       if (G.J > 1) {             // partial result of this dy chunk; k1_fast_merge_kernel finishes the pixel
         const size_t pk = ((size_t)chunk * G.H + gy) * G.W + gx;
@@ -585,19 +451,13 @@ int k1_fast_launch(int cost, ImgF left, ImgF right, int W, int H, int sx, int sy
   FastGeom g = fast_geom(W, H, sx, sy, kx, ky);
   g.scale = sq ? 1 : F_B;
   if (org) { g.lox = org->lox; g.loy = org->loy; g.rox = org->rox; g.roy = org->roy; g.addx = org->addx; g.addy = org->addy; }
-  // fp32 carries the integers exactly while every window sum * 8 (+7) stays below 2^24
-  // variants: all-int (default, ALU-pipe bound), int with fp32 seeding (VWB200_K1_FAST=fseed), all-fp32 on the FMA
-  // pipes (VWB200_K1_FAST=float; issue-bound).  All three are exact.
-  const char* mode = getenv("VWB200_K1_FAST");
-  const bool float_ok = (double)(vmax - vmin) * kx * ky * F_B + F_B < 16777216.0;
-  const bool fseed_ok = (double)(vmax - vmin) * ky * F_B < 8388608.0;
-  const bool use_float = float_ok && mode && !strcmp(mode, "float");
-  const bool float_seed = fseed_ok && mode && !strcmp(mode, "fseed");     // issue-bound like all-int
   unsigned char* ws = static_cast<unsigned char*>(workspace);
   uint16_t* L16 = reinterpret_cast<uint16_t*>(ws);
   uint16_t* R16 = L16 + (size_t)g.NS * g.lrows * F_COLS;
   uint32_t* part_cost = reinterpret_cast<uint32_t*>((reinterpret_cast<uintptr_t>(R16 + (size_t)g.NS * g.rrows * g.rw) + 63) & ~(uintptr_t)63);
   uint16_t* part_idx = reinterpret_cast<uint16_t*>(part_cost + (size_t)g.J * W * H);
+  const uintptr_t kbase = g.J > 1 ? reinterpret_cast<uintptr_t>(part_idx + (size_t)g.J * W * H) : reinterpret_cast<uintptr_t>(part_cost);
+  unsigned long long* gkeys = reinterpret_cast<unsigned long long*>((kbase + 63) & ~(uintptr_t)63);
   {
     dim3 gl(g.lrows, g.NS), gr(g.rrows, g.NS);
     pack_left_kernel<<<gl, 256, 0, st>>>(left, vmin, g, L16);
@@ -609,11 +469,11 @@ int k1_fast_launch(int cost, ImgF left, ImgF right, int W, int H, int sx, int sy
   VWB_CUDA(cudaGetDevice(&dev));
   VWB_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
   const int items = g.NS * g.NB * g.J;
-  const int grid = items < nsm ? items : nsm;
+  const int grid = std::min(items, std::min(nsm, kNumSMs));      // the workspace holds kNumSMs key planes
   const size_t smem = fast_smem_bytes(g);
-  void (*kern)(const uint16_t*, const uint16_t*, FastGeom, vwb200_dispi*, ptrdiff_t, uint32_t*, uint16_t*) = nullptr;
+  void (*kern)(const uint16_t*, const uint16_t*, FastGeom, vwb200_dispi*, ptrdiff_t, uint32_t*, uint16_t*, unsigned long long*) = nullptr;
   switch (kx) {
-#define KCASE(K) case K: kern = sq ? k1_fast_abs_kernel<K, false, false, true> : (use_float ? k1_fast_abs_kernel<K, true, false> : (float_seed ? k1_fast_abs_kernel<K, false, true> : k1_fast_abs_kernel<K, false, false>)); break;
+#define KCASE(K) case K: kern = sq ? k1_fast_abs_kernel<K, true> : k1_fast_abs_kernel<K, false>; break;
     KCASE(3) KCASE(5) KCASE(7) KCASE(9) KCASE(11) KCASE(13) KCASE(15) KCASE(17) KCASE(19) KCASE(21) KCASE(23) KCASE(25)
     KCASE(27) KCASE(29) KCASE(31)
 #undef KCASE
@@ -621,7 +481,7 @@ int k1_fast_launch(int cost, ImgF left, ImgF right, int W, int H, int sx, int sy
   }
   VWB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FK_SMEM));   // per-function state shared by all host threads: device maximum
   if (ev && ev->e0) cudaEventRecord(ev->e0, st);
-  kern<<<grid, F_THREADS, smem, st>>>(L16, R16, g, out, opitch, part_cost, part_idx);
+  kern<<<grid, F_THREADS, smem, st>>>(L16, R16, g, out, opitch, part_cost, part_idx, gkeys);
   VWB_LAUNCH_CHECK();
   if (ev && ev->e1) cudaEventRecord(ev->e1, st);
   if (g.J > 1) {
