@@ -32,13 +32,19 @@
 namespace vwb200 {
 
 // ---- min / max / integer-valuedness reduction -------------------------------------------------------
+// order-preserving float -> int key so that integer atomics can be used; taken from the sign bit, so -0.0 and +0.0 both
+// map to 0 (a key from `v >= 0` would send -0.0 to INT_MIN, below every negative pixel).  image_stats_fini inverts it.
+static __device__ __forceinline__ int stats_key(float v) {
+  const int b = __float_as_int(v);
+  return b >= 0 ? b : (int)(0x80000000u - (unsigned)b);
+}
 __global__ void image_stats_kernel(ImgF img, float* __restrict__ result) {
   float mn = INFINITY, mx = -INFINITY; int allint = 1;
   const long long n = (long long)img.w * img.h;
   for (long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (long long)gridDim.x * blockDim.x) {
     const float v = img.p[(ptrdiff_t)(k / img.w) * img.pitch + (k % img.w)];
     mn = fminf(mn, v); mx = fmaxf(mx, v);
-    if (!(v == rintf(v))) allint = 0;          // NaN/inf -> not integer
+    if (!isfinite(v) || v != rintf(v)) allint = 0;          // NaN/inf -> not integer
   }
   for (int o = 16; o > 0; o >>= 1) {
     mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
@@ -46,9 +52,8 @@ __global__ void image_stats_kernel(ImgF img, float* __restrict__ result) {
     allint &= __shfl_xor_sync(0xffffffffu, allint, o);
   }
   if ((threadIdx.x & 31) == 0) {
-    // order-preserving float->int mapping so integer atomics can be used
-    atomicMin(reinterpret_cast<int*>(result) + 0, mn >= 0 ? __float_as_int(mn) : (int)(0x80000000u - (unsigned)__float_as_int(mn)));
-    atomicMax(reinterpret_cast<int*>(result) + 1, mx >= 0 ? __float_as_int(mx) : (int)(0x80000000u - (unsigned)__float_as_int(mx)));
+    atomicMin(reinterpret_cast<int*>(result) + 0, stats_key(mn));
+    atomicMax(reinterpret_cast<int*>(result) + 1, stats_key(mx));
     if (!allint) atomicExch(reinterpret_cast<int*>(result) + 2, 0);
   }
 }
