@@ -132,6 +132,10 @@ int vwb200_parabola_subpixel(const float* disparity, int cols, int rows, const f
  * range).  Disparities lie in [0, search_x] x [0, search_y] (inclusive = search_volume of the reference).
  * out receives out_w x out_h pixels (row pitch opitch elements; the size is (:2397-2420) and can be queried first
  * with all outputs NULL).
+ * Penalties: after the defaults are applied (p1 / p2 <= 0), every entry point needs p1 <= p2 <= 30000 and returns
+ * VWB200_ENOIMPL otherwise, with both values in vwb200_last_error().  This is stricter than the reference, which takes
+ * any uint16 pair (SGM.cc:77-160): a given p2 below the default p1 (census 7 with p1 = 0, p2 = 29) is refused too.
+ * Inside the range, accumulated costs above 65535 wrap around in uint16 exactly as the reference's do.
  * ------------------------------------------------------------------------------------------- */
 /* the simple form: the same search box for every pixel (populate_constant_disp_bound_image, :231-239), plain
  * census costs, no masks, no previous disparity; p1 / p2 <= 0 select the reference's defaults (:108-157) */
@@ -155,7 +159,8 @@ typedef struct {
   int32_t cost_type;                     /* VWB200_CENSUS_TRANSFORM or VWB200_TERNARY_CENSUS_TRANSFORM; anything else:
                                             VWB200_ENOIMPL like SGM.cc:1888-1892 */
   int32_t ternary_threshold;             /* ternary_census_threshold (default 5) */
-  int32_t p1, p2;                        /* <= 0: the reference's defaults for the cost type and kernel */
+  int32_t p1, p2;                        /* <= 0: the reference's defaults for the cost type and kernel; then
+                                            p1 <= p2 <= 30000, else VWB200_ENOIMPL */
   int32_t use_mgm;
   int32_t subpixel_mode;
   int32_t search_buffer_x, search_buffer_y;   /* sgm_search_buffer, applied around the doubled previous disparity */

@@ -2,23 +2,26 @@
  *
  * TEST INFRASTRUCTURE ONLY (see oracle/vw_oracle.h): nothing under visionworkbench_b200/ may use it.
  *
- * Scope of this first cut (round 1): vw::stereo::calc_disparity_sgm (Stereo/SGM.cc:167-230) ->
- * SemiGlobalMatcher::semi_global_matching_func (:2387-2448) with
- *   - CENSUS_TRANSFORM costs, kernel 3/5/7/9 (Image/CensusTransform.h:64-160, SGM.cc:39-73,1740-1873),
- *   - the same search box for every pixel (populate_constant_disp_bound_image, :231-239): no masks, no previous disparity,
+ * Scope: vw::stereo::calc_disparity_sgm (Stereo/SGM.cc:167-230) -> SemiGlobalMatcher::semi_global_matching_func
+ * (:2387-2448) with
+ *   - CENSUS_TRANSFORM and TERNARY_CENSUS_TRANSFORM costs, kernel 3/5/7/9 (Image/CensusTransform.h:64-340,
+ *     SGM.cc:39-73,1740-1873),
+ *   - explicit penalties p1 / p2 (set_parameters, :77-160; <= 0 selects the defaults),
+ *   - the same search box for every pixel (populate_constant_disp_bound_image, :231-239),
  *   - plain SGM accumulation along 8 directions (accum_sgm_multithread, :2462-2611; PixelPassTask, SGMAssist.h:691-832)
  *     with the SSE flavour of evaluate_path (:1014-1141, compute_path_internals_sse :950-990: unsigned 16-bit min,
  *     SATURATING add / subtract) -- the reference is built with SSE4.1, and the scalar flavour (:806-913) differs on overflow,
  *   - the integer winner of select_best_disparity (:1159-1288, including its tie-smoothing iterations that rewrite the
  *     accumulated costs) as used by create_disparity_view (:1290-1346),
- *   - the 1-D sub-pixel models of create_disparity_view_subpixel (:1402-1480,1497-1614; every SgmSubpixelMode but the 2-D
- *     parabola).
- * Further down: the same pipeline with a search box per pixel (vwo_sgm_calc_disparity_bounds) and the derivation of those
+ *   - the sub-pixel models of create_disparity_view_subpixel (:1402-1480,1497-1614), the 2-D parabola included.
+ * Further down: the same pipeline with a search box per pixel (vwo_sgm_calc_disparity_bounds), the derivation of those
  * boxes from masks and the previous pyramid level (vwo_sgm_disp_bounds: populate_disp_bound_image / constrain_disp_bound_image,
- * :241-668) -- oracle only so far, the device side is round-2 work.
- * and MGM accumulation (vwo_mgm_calc_disparity_bounds).  Not restated yet: ternary census, the memory-limit retry loop
- * (:476-497), the 2-D parabola sub-pixel mode, the R->L / filtering glue of CorrelationView.cc:360-590.  Pinned by TestSGM.cxx:27-75 (> 99 % of the pixels equal the true constant offset) on the reference's own
- * fixture images; the sub-pixel stage has no known-answer test in the reference (floats: tolerance 1e-5 on the GPU side).
+ * :241-668) with the memory-limit retry loop over the conservation levels (:476-497), MGM accumulation
+ * (vwo_mgm_calc_disparity_bounds), and the whole entry point (vwo_calc_disparity_sgm).  The R->L / filtering glue of
+ * CorrelationView.cc:360-590 lives in vw_oracle.c.  Pinned by TestSGM.cxx:27-75 (> 99 % of the pixels equal the true
+ * constant offset) on the reference's own fixture images, and, across the penalty range, by an independent numpy
+ * restatement (tests/sgm_reference.py, tests/test_oracle_sgm_penalties.py); the sub-pixel stage has no known-answer test in
+ * the reference (floats: tolerance 1e-5 on the GPU side).
  *
  * The accumulation order of the reference is thread dependent but irrelevant: every pixel lies on exactly one line per
  * direction and the per-line results are ADDED (uint16, wrapping) into the accumulation buffer (SGMAssist.h:790-815).
