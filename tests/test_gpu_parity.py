@@ -398,7 +398,7 @@ def test_calc_disparity_exact_int_fast_path_squared(vwb, oracle, shape):
 @pytest.mark.parametrize("shape", [((300, 70), (16, 8), (21, 21)), ((260, 100), (33, 5), (7, 7)), ((473, 65), (24, 11), (15, 9)),
                                    ((64, 64), (8, 8), (3, 5)), ((250, 40), (128, 2), (21, 21))])
 def test_calc_disparity_exact_int_fast_path_ncc(vwb, oracle, shape):
-    """NCC on the exact-integer kernel (k1_fast_ncc): integer numerators, fp32 upper-bound screening, exact double
+    """NCC on the exact-integer kernel (k1_screen): integer numerators, fp32 upper-bound screening, exact double
     evaluation (reference arithmetic) of the surviving candidates."""
     from visionworkbench_b200.synth import make_rasters
     (W, H), search, kernel = shape

@@ -922,7 +922,7 @@ static int calc_disparity_device(int cost_type, ImgF Li, ImgF Ri, int W, int H, 
     VWB_TRY(ar.alloc(&ws, wb));
     VWB_TRY(k1_fast_launch(cost_type, Li, Ri, W, H, sx, sy, kx, ky, vmin, vmax, dout, dop, ws, wb, st, kev));
     path = 0;
-  } else if (k1_screen_supported(cost_type, kx, ky, sx, sy, vmin, vmax, integer) == VWB200_OK && !getenv("VWB200_K1_GENERIC")) {
+  } else if (k1_screen_supported(cost_type, kx, ky, sx, sy, vmin, vmax, integer) == VWB200_OK) {
     unsigned char* ws;
     VWB_TRY(ar.alloc(&ws, k1_screen_workspace_bytes(cost_type, W, H, sx, sy, kx, ky)));
     VWB_TRY(k1_screen_launch(cost_type, Li, Ri, W, H, sx, sy, kx, ky, vmin, vmax, dout, dop, ws, st, kev));

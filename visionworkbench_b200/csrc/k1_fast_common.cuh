@@ -1,5 +1,5 @@
 // k1_fast_common.cuh -- pieces shared by the exact-integer fast kernels (k1_fast.cu: AbsoluteCost / SquaredCost,
-// k1_fast_ncc.cu: NCC): tile geometry, mbarrier + TMA bulk-copy PTX wrappers, shuffle-based window sums.
+// k1_screen.cu: NCC and SquaredCost screening): tile geometry, mbarrier + TMA bulk-copy PTX wrappers, shuffle-based window sums.
 #pragma once
 #include "common.cuh"
 
@@ -7,10 +7,7 @@ namespace vwb200 {
 
 static constexpr int F_TH = 32;        // output rows per band of k1_screen (k1_fast: FastGeom::th)
 static constexpr int F_COLS = 256;     // padded columns per strip (32 lanes x 8)
-static constexpr int F_WARPS = 8;       // per CTA (2 per SM sub-partition); k1_screen: 4 dx subsets x 2 row halves
-static constexpr int F_SUBSETS = 4;
-static constexpr int F_HALVES = F_WARPS / F_SUBSETS;
-static constexpr int F_RH = F_TH / F_HALVES;      // output rows per warp
+static constexpr int F_WARPS = 8;       // per CTA (2 per SM sub-partition)
 static constexpr int F_THREADS = F_WARPS * 32;
 static constexpr int F_B = 8;          // consecutive dx per thread (one "octet"); keys are cost*8 + b
 
@@ -28,7 +25,6 @@ struct FastGeom {
   int lox, loy, rox, roy;   // origin of the (logical) left / right rasters inside the images passed to the pack kernels
   int addx, addy;           // constant added to the output disparities
   int sd;                   // k1_screen: dy rows per synchronisation period (ring depth)
-  int dynamic_units;          // k1_screen: 1 = warps draw (octet, half) work units from a shared counter, 0 = static round-robin
   int th;                   // output rows per band (F_TH for k1_screen; k1_fast sizes it from its shared-memory budget)
 };
 static inline FastGeom make_geom(int W, int H, int sx, int sy, int kx, int ky, int th = F_TH) {
@@ -42,7 +38,7 @@ static inline FastGeom make_geom(int W, int H, int sx, int sy, int kx, int ky, i
   g.lrows = g.NB * th + ky - 1;
   g.rrows = g.NB * th + ky - 1 + sy;
   g.rw = ((F_COLS + sx + 7) / 8) * 8 + 8;
-  g.lox = g.loy = g.rox = g.roy = 0; g.addx = g.addy = 0; g.scale = F_B; g.dynamic_units = 1; g.sd = 1;
+  g.lox = g.loy = g.rox = g.roy = 0; g.addx = g.addy = 0; g.scale = F_B; g.sd = 1;
   // The work items (strip x band x dy-chunk) are dealt round-robin to kNumSMs persistent CTAs, so the last partial wave idles
   // part of the chip: 1120 items = 8.48 waves run as 9 (efficiency 0.943 -- the 8-GPU share of the 8192^2 raster).  Split
   // the dy range into J chunks (merged by k1_fast_merge) so that items * J fills its last wave: pick the J with the best

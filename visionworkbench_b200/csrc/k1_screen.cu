@@ -34,6 +34,8 @@
 namespace vwb200 {
 
 enum { M_NCC = 0, M_SQ = 1 };
+static constexpr int S_HALVES = 2;               // a band is screened in row halves: work unit = (dy, dx octet, half)
+static constexpr int S_RH = F_TH / S_HALVES;     // output rows per work unit
 static constexpr int SD_MAX = 3;                 // dy rows per synchronisation period (ring depth): fewer, cheaper barriers
 static inline __host__ __device__ int nq_slots(int sd) { return F_TH + 2 * sd - 1; }
 static constexpr float QI_ZERO = 1.0e-30f;      // Qi of a zero-energy right window (its cost is NaN)
@@ -363,7 +365,7 @@ __device__ __forceinline__ void screen_pass(const int16_t* __restrict__ ltile, c
   }
   int slot_old = ring_base;
   int qslot = qbase;                       // ring slot of the right window-origin row (dy + row0 + y)
-  for (int y = 0; y < F_RH; ++y) {
+  for (int y = 0; y < S_RH; ++y) {
     if (y > 0) {
       {
         int Lv[8], Rv[16];
@@ -536,8 +538,8 @@ k1_screen_kernel(const int16_t* __restrict__ L16, const int16_t* __restrict__ R1
   uint64_t* bars = reinterpret_cast<uint64_t*>(aring + (size_t)(MODE == M_NCC ? 2 : 1) * NQ_SLOTS * G.rw);
   CandCtx* cc = reinterpret_cast<CandCtx*>(bars + 2);
   const uint32_t c_sa = smem_u32(cc);
-  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-  const int ngroups = (G.sx + F_B - 1) / F_B, nunits = ngroups * F_HALVES;
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int ngroups = (G.sx + F_B - 1) / F_B, nunits = ngroups * S_HALVES;
   unsigned long long* bk = bk_all + (size_t)blockIdx.x * F_TH * F_COLS;
   int* bi = bi_all + (size_t)blockIdx.x * F_TH * F_COLS;
   uint4* list = list_all + (size_t)blockIdx.x * cap;
@@ -600,18 +602,13 @@ k1_screen_kernel(const int16_t* __restrict__ L16, const int16_t* __restrict__ R1
       }
       // work units of this period = (dy, dx octet, row half); warps draw them from a shared counter: unit durations
       // differ (candidate handling around the cost peak), a static split leaves warps waiting at the barrier
-      for (int uu = 0;; ++uu) {
-        int u;
-        if (G.dynamic_units) {
-          u = 0;
-          if (lane == 0) u = atoms_add_s32(c_sa + (uint32_t)offsetof(CandCtx, next) + 4u * (per & 1), 1);
-          u = __shfl_sync(0xffffffffu, u, 0);
-        } else {
-          u = w + F_WARPS * uu;                            // static round-robin: unit u -> (octet u % ngroups, half u / ngroups)
-        }
+      for (;;) {
+        int u = 0;
+        if (lane == 0) u = atoms_add_s32(c_sa + (uint32_t)offsetof(CandCtx, next) + 4u * (per & 1), 1);
+        u = __shfl_sync(0xffffffffu, u, 0);
         if (u >= nunits * dcur) break;
         const int dy = dyp + u / nunits, uu2 = u % nunits;
-        const int g = uu2 % ngroups, row0 = (uu2 / ngroups) * F_RH;
+        const int g = uu2 % ngroups, row0 = (uu2 / ngroups) * S_RH;
         const int ring_base = (dy + row0) % G.ring_slots;
         const int qbase = (dy + row0) % NQ_SLOTS;
         if (G.sx - F_B * g >= F_B)
@@ -711,7 +708,6 @@ static int screen_launch_t(ImgF left, ImgF right, int W, int H, int sx, int sy, 
   if (!screen_geom(g, MODE)) { set_error("k1_screen: search width %d does not fit in shared memory", sx); return VWB200_ENOIMPL; }
   g.scale = 1;
   if (org) { g.lox = org->lox; g.loy = org->loy; g.rox = org->rox; g.roy = org->roy; g.addx = org->addx; g.addy = org->addy; }
-  g.dynamic_units = getenv("VWB200_SCREEN_DYNAMIC") ? atoi(getenv("VWB200_SCREEN_DYNAMIC")) : 1;
   int c; double maxc;
   if (!screen_params(MODE, kx, ky, vmin, vmax, &c, &maxc)) { set_error("k1_screen: unsupported value range"); return VWB200_ENOIMPL; }
   const ScreenWs ws = carve(g, MODE, workspace);
@@ -743,7 +739,7 @@ static int screen_launch_t(ImgF left, ImgF right, int W, int H, int sx, int sy, 
   }
   // seeding stage (skipped when the half-resolution problem is outside what k1_fast handles)
   const float* T0 = nullptr;
-  if (!getenv("VWB200_SCREEN_NOSEED") && W >= 64 && H >= 64 &&
+  if (W >= 64 && H >= 64 &&
       k1_fast_supported(VWB200_ABSOLUTE_DIFFERENCE, ws.kx2, ws.ky2, ws.sx2, ws.sy2, vmin, vmax, true) == VWB200_OK) {
     const int lw2 = ws.W2 + ws.kx2 - 1, lh2 = ws.H2 + ws.ky2 - 1, rw2 = lw2 + ws.sx2 - 1, rh2 = lh2 + ws.sy2 - 1;
     dim3 b2(32, 8);

@@ -295,9 +295,9 @@ __global__ void __launch_bounds__(256) sgm_meta_kernel(const short4* __restrict_
 // ---- Hamming costs (get_hamming_distance_costs, SGM.cc:39-73) ---------------------------------------------------------
 // one warp per 32 consecutive pixels: lane i fetches record i (coalesced), then the warp walks the 32 pixels with
 // lanes = the pixel's disparities (coalesced byte stores into the ragged volume); 4 pixels in flight per iteration
-// only_big != 0: the warps whose 32 pixels all have <= 32 entries were done by sgm_cost_lanes_kernel
+// The warps whose 32 pixels all have <= 32 entries were done by sgm_cost_lanes_kernel.
 __global__ void __launch_bounds__(256) sgm_cost_kernel(const unsigned long long* __restrict__ lc, const unsigned long long* __restrict__ rc,
-                                                       const SgmMeta* __restrict__ meta, SgmGeom g, sgm_cost_t* __restrict__ cost, int only_big) {
+                                                       const SgmMeta* __restrict__ meta, SgmGeom g, sgm_cost_t* __restrict__ cost) {
   const int lane = threadIdx.x & 31;
   const size_t npix = (size_t)g.ow * g.oh;
   const size_t p0 = (((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5) * 32;
@@ -307,7 +307,7 @@ __global__ void __launch_bounds__(256) sgm_cost_kernel(const unsigned long long*
   unsigned long long l = 0;
   int br = 0, bc = 0;
   if (mine < npix) mq = __ldg(reinterpret_cast<const uint4*>(meta) + mine);
-  if (only_big && !__any_sync(0xffffffffu, (mq.w >> 8) > 32u)) return;
+  if (!__any_sync(0xffffffffu, (mq.w >> 8) > 32u)) return;
   if (mine < npix) {
     const int c = (int)(mine % g.ow), r = (int)(mine / g.ow);
     br = r + g.min_row - g.hk; bc = c + g.min_col - g.hk;
@@ -355,7 +355,7 @@ __global__ void __launch_bounds__(256) sgm_cost_lanes_kernel(const unsigned long
   uint4 mq = make_uint4(0xffff0000u, 0xffffu, 0u, 0u);
   if (mine < npix) mq = __ldg(reinterpret_cast<const uint4*>(meta) + mine);
   const unsigned n = mine < npix ? (mq.w >> 8) : 0u;
-  if (__any_sync(0xffffffffu, n > 32u)) return;                          // sgm_cost_kernel(only_big) takes this warp
+  if (__any_sync(0xffffffffu, n > 32u)) return;                          // sgm_cost_kernel takes this warp
   const unsigned st0 = __shfl_sync(0xffffffffu, mq.z, 0);                 // pixel p0 always exists
   unsigned end = n ? mq.z + n : st0;
   for (int o = 16; o > 0; o >>= 1) end = max(end, __shfl_xor_sync(0xffffffffu, end, o));
@@ -448,17 +448,16 @@ __global__ void __launch_bounds__(256) sgm_sum4_kernel(uint4* __restrict__ a0, c
   }
 }
 
-// accum = the first partial volume (it receives the totals of the pixels that need them re-read: ties, sub-pixel), a1..a3 =
-// the other partial volumes of the concurrent directions (NULL: accum already holds the total)
-// staged != 0 (with a1..a3): a warp's 32 consecutive pixels own one contiguous range of the ragged volumes; when every one of
-// them has <= 32 entries the warp adds the four partial volumes with coalesced word loads into shared memory and the
-// winner / sub-pixel stages read the totals from there (nothing is written back unless a pixel needs the tie smoothing).
+// accum = the first partial volume (it receives the totals of the pixels that need the tie smoothing), a1..a3 = the other
+// partial volumes of the concurrent directions (NULL: accum already holds the total).
+// With a1..a3, EVERY pixel must have <= 32 entries: a warp's 32 consecutive pixels own one contiguous range of the ragged
+// volumes, which the warp adds with coalesced word loads into shared memory, and the winner / sub-pixel stages read the
+// totals from there (nothing is written back unless a pixel needs the tie smoothing).
 __global__ void __launch_bounds__(128) sgm_wta_kernel(sgm_accum_t* __restrict__ accum, const sgm_accum_t* __restrict__ a1,
                                                       const sgm_accum_t* __restrict__ a2, const sgm_accum_t* __restrict__ a3,
                                                       sgm_accum_t* __restrict__ scratch,
                                                       const SgmMeta* __restrict__ meta, SgmGeom g, vwb200_dispi* __restrict__ out,
-                                                      ptrdiff_t opitch, int want_sub, int mode, float* __restrict__ out_sub, ptrdiff_t sub_pitch,
-                                                      int staged) {
+                                                      ptrdiff_t opitch, int want_sub, int mode, float* __restrict__ out_sub, ptrdiff_t sub_pitch) {
   __shared__ __align__(16) sgm_accum_t tot[4][1024 + 8];
   const size_t pix = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   const size_t npix = (size_t)g.ow * g.oh;
@@ -467,7 +466,7 @@ __global__ void __launch_bounds__(128) sgm_wta_kernel(sgm_accum_t* __restrict__ 
   if (pix < npix) mq = __ldg(reinterpret_cast<const uint4*>(meta) + pix);
   const int num = pix < npix ? (int)(mq.w >> 8) : 0;
   const sgm_accum_t* tot_vec = nullptr;                                 // != NULL: this pixel's totals in shared memory
-  if (staged && a1 && !__any_sync(0xffffffffu, num > 32)) {
+  if (a1) {
     const unsigned st0 = __shfl_sync(0xffffffffu, mq.z, 0);              // the warp's first pixel exists (pix - lane < npix)
     unsigned end = num ? mq.z + (unsigned)num : st0;
     for (int o = 16; o > 0; o >>= 1) end = max(end, __shfl_xor_sync(0xffffffffu, end, o));
@@ -497,22 +496,14 @@ __global__ void __launch_bounds__(128) sgm_wta_kernel(sgm_accum_t* __restrict__ 
   const int width = b2 - b0 + 1, height = b3 - b1 + 1;
   int min_count = 0, min_index = 0;
   unsigned min_val = 65535;
-  const bool parts = a1 != nullptr && !tot_vec;
-  const bool need_total = parts && want_sub && mode != 0;              // the sub-pixel stage re-reads neighbours of the winner
   for (int i = 0; i < num; ++i) {
-    unsigned v = tot_vec ? tot_vec[i] : accum_vec[i];
-    if (parts) {                                                        // uint16 wrapping sum, like the reference's in-place adds
-      v = (v + a1[mq.z + i] + a2[mq.z + i] + a3[mq.z + i]) & 0xffffu;
-      if (need_total) accum_vec[i] = (sgm_accum_t)v;
-    }
+    const unsigned v = tot_vec ? tot_vec[i] : accum_vec[i];
     if (v == min_val) ++min_count;
     if (v < min_val) { min_index = i; min_val = v; min_count = 1; }
   }
   bool in_global = !tot_vec;                                            // where the totals of this pixel are
   if (min_count > 1) {                                                  // tie smoothing (:1196-1288), rare
     if (tot_vec) { for (int i = 0; i < num; ++i) accum_vec[i] = tot_vec[i]; in_global = true; }
-    if (parts && !need_total)
-      for (int i = 0; i < num; ++i) accum_vec[i] = (sgm_accum_t)((accum_vec[i] + a1[mq.z + i] + a2[mq.z + i] + a3[mq.z + i]) & 0xffffu);
     for (int i = 0; i < num; ++i) buffer[i] = accum_vec[i];
     sgm_accum_t* input_array = accum_vec;
     sgm_accum_t* output_array = buffer;
@@ -800,12 +791,9 @@ int sgm_run(const SgmArgs& a, Arena& /*callers_arena*/, cudaStream_t st) {
     parts[k] += 64;
   }
   static_assert(sizeof(sgm_cost_t) == 1, "the staged copy moves bytes");
-  const int lanes_path = getenv("VWB200_SGM_COST_OLD") ? 0 : 1;
-  if (lanes_path) {
-    sgm_cost_lanes_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, st>>>(lc, rc, meta, g, cost);
-    VWB_LAUNCH_CHECK();
-  }
-  sgm_cost_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, st>>>(lc, rc, meta, g, cost, lanes_path);
+  sgm_cost_lanes_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, st>>>(lc, rc, meta, g, cost);
+  VWB_LAUNCH_CHECK();
+  sgm_cost_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, st>>>(lc, rc, meta, g, cost);
   VWB_LAUNCH_CHECK();
   VWB_CUDA(cudaStreamSynchronize(st));                                  // max_n
   if (a.use_mgm) {
@@ -814,7 +802,7 @@ int sgm_run(const SgmArgs& a, Arena& /*callers_arena*/, cudaStream_t st) {
   } else {
     VWB_TRY(sgm_paths_launch(meta, cost, parts, naccum, g, maxes[0], maxes[1], maxes[2], ar, st));
   }
-  const bool fused_wta = naccum == 4 && maxes[0] <= 32 && !getenv("VWB200_SGM_WTA_UNFUSED");   // every pixel has <= 32 entries
+  const bool fused_wta = naccum == 4 && maxes[0] <= 32;   // every pixel has <= 32 entries: sgm_wta_kernel adds the partial volumes
   if (naccum == 4 && !fused_wta) {
     const size_t nvec = ((size_t)total + 7) / 8;              // the volumes are 16-byte aligned and padded
     sgm_sum4_kernel<<<kNumSMs * 8, 256, 0, st>>>(reinterpret_cast<uint4*>(accum), reinterpret_cast<const uint4*>(parts[1]),
@@ -823,7 +811,7 @@ int sgm_run(const SgmArgs& a, Arena& /*callers_arena*/, cudaStream_t st) {
   }
   sgm_wta_kernel<<<(unsigned)((npix + 127) / 128), 128, 0, st>>>(accum, fused_wta ? parts[1] : nullptr, fused_wta ? parts[2] : nullptr,
                                                                  fused_wta ? parts[3] : nullptr, scratch, meta, g, a.out, a.opitch,
-                                                                 a.out_sub != nullptr, a.subpixel_mode, a.out_sub, a.sub_pitch, fused_wta ? 1 : 0);
+                                                                 a.out_sub != nullptr, a.subpixel_mode, a.out_sub, a.sub_pitch);
   VWB_LAUNCH_CHECK();
   return VWB200_OK;
 }
