@@ -4,6 +4,8 @@ reference's order with no FMA contraction)."""
 import numpy as np
 import pytest
 
+from kernel_trace import trace  # noqa: F401  (the profiler fixture: the kernels a call ran)
+
 pytestmark = pytest.mark.gpu
 
 
@@ -349,13 +351,19 @@ def test_parabola_subpixel_reference_kat(vwb):
     assert err < 0.6 and err < np.abs(np.rint(true) - true)[10:100].mean()
 
 
-def test_generic_kernel_unsplit_large_search(vwb, oracle, monkeypatch):
-    """A zone whose partial-result scratch would be too large is NOT split over disparity chunks: the single CTA
-    loop must then cover the whole search range (regression: it covered only the first 256 disparities)."""
+def test_generic_kernel_unsplit_large_search(vwb, oracle, trace):
+    """1200 disparities on float imagery: the generic kernel splits the zone into five chunks of 256 disparities
+    (40 * 24 * 5 partial results are far below the 2^29 scratch limit) and k1_generic_merge_kernel must find the matches
+    that lie beyond the first chunk (regression: a CTA covered only the first 256 disparities).  An unsplit zone of this
+    many disparities needs a scratch of 2^29 elements, beyond what a test raster here reaches."""
     from visionworkbench_b200.synth import make_rasters
-    W, H, search, kernel = 40, 24, (40, 30), (5, 5)       # 1200 disparities, SquaredCost -> generic kernel
+    W, H, search, kernel = 40, 24, (40, 30), (5, 5)
     left, right = make_rasters(W, H, search, kernel, seed=77)
-    got = vwb.calc_disparity(1, left, right, search, kernel)
+    left, right = left + 0.5, right + 0.5                   # not integer valued: the generic kernel, same SquaredCost costs
+    got = trace.run(lambda: vwb.calc_disparity(1, left, right, search, kernel))
+    exp = trace.assert_hot(1, left, right, search, kernel)
+    assert exp.family == "k1_generic_kernel" and exp.geom["nchunks"] == 5
+    assert [k[0] for k in trace.merges()] == ["k1_generic_merge_kernel"]
     ref = oracle.calc_disparity(1, left, right, search, kernel)
     _assert_disp_equal(got, ref)
     assert (ref[..., 0] + ref[..., 1] * 40).max() > 256     # the true matches lie beyond the first chunk
@@ -379,13 +387,16 @@ def test_view_single_level_uses_fast_kernel(vwb, oracle, consistency):
 
 
 @pytest.mark.parametrize("shape", [((300, 70), (16, 8), (21, 21)), ((260, 100), (33, 5), (7, 7)), ((473, 65), (24, 11), (15, 9))])
-def test_calc_disparity_exact_int_fast_path_squared(vwb, oracle, shape):
-    """SquaredCost on the exact-integer kernel: uint32 window sums, compare/select arg-min."""
+def test_calc_disparity_exact_int_fast_path_squared(vwb, oracle, trace, shape):
+    """SquaredCost on K1 fast: uint32 window sums, compare/select arg-min.  The imagery is capped at 3000 so that every
+    shape stays on K1 fast (441 * 3000^2 < 2^32 at 21 x 21; a range of 3121 or more would take K1 screen)."""
     from visionworkbench_b200.synth import make_rasters
     (W, H), search, kernel = shape
     left, right = make_rasters(W, H, search, kernel, seed=17 + W)
-    got = vwb.calc_disparity(1, left, right, search, kernel)
+    left, right = np.minimum(left, 3000.0), np.minimum(right, 3000.0)
+    got = trace.run(lambda: vwb.calc_disparity(1, left, right, search, kernel))
     assert vwb.last_k1_stats()["path"] == "exact-int"
+    assert trace.assert_hot(1, left, right, search, kernel).family == "k1_fast_abs_kernel"
     _assert_disp_equal(got, oracle.calc_disparity(1, left, right, search, kernel), f"fast sq {shape}")
     # range too large for uint32 sums -> general kernel, same answer
     big = left * 16.0
@@ -428,15 +439,19 @@ def test_fast_ncc_ties_zero_windows_and_constant_regions(vwb, oracle):
 
 @pytest.mark.parametrize("shape", [((300, 70), (16, 8), (21, 21)), ((260, 100), (33, 5), (7, 7)), ((250, 40), (128, 2), (21, 21)),
                                    ((64, 64), (8, 8), (3, 5))])
-def test_calc_disparity_screened_squared_12bit(vwb, oracle, shape):
-    """SquaredCost whose window sums exceed uint32 (12-bit imagery, 21x21) takes the screened exact-integer kernel
-    (k1_screen): centred int32 numerators, fp32 screening, exact int64 evaluation of the surviving candidates."""
+def test_calc_disparity_screened_squared_12bit(vwb, oracle, trace, shape):
+    """SquaredCost on 12-bit imagery with the full range 4095.  At 21 x 21 the window sums exceed uint32 and the screened
+    exact-integer kernel (k1_screen) runs: centred int32 numerators, fp32 screening, exact int64 evaluation of the
+    surviving candidates.  The 7 x 7 and 3 x 5 shapes fit uint32 (Sq on K1 screen needs kx * ky >= 257) and test K1 fast."""
     from visionworkbench_b200.synth import make_rasters
     (W, H), search, kernel = shape
     left, right = make_rasters(W, H, search, kernel, seed=5 + W, bits=12)
+    left[0, 0], left[0, 1] = 0.0, 4095.0                # the full 12-bit range, whatever the smoothing left
     left = left - 700.0; right = right - 700.0          # SquaredCost only needs a bounded range, not non-negative values
-    got = vwb.calc_disparity(1, left, right, search, kernel)
+    got = trace.run(lambda: vwb.calc_disparity(1, left, right, search, kernel))
     assert vwb.last_k1_stats()["path"] == "exact-int"
+    family = trace.assert_hot(1, left, right, search, kernel).family
+    assert family == ("k1_screen_kernel" if kernel[0] * kernel[1] >= 257 else "k1_fast_abs_kernel")
     ref = oracle.calc_disparity(1, left, right, search, kernel)
     _assert_disp_equal(got, ref, f"screened sq {shape}")
 

@@ -8,6 +8,8 @@ packing of every exact kernel and SGM's u8_convert stretch.  Every case here is 
 import numpy as np
 import pytest
 
+from kernel_trace import trace  # noqa: F401  (the profiler fixture: the kernels a call ran)
+
 pytestmark = pytest.mark.gpu
 
 EXACT, FP64 = "exact-int", "general-fp64"
@@ -79,12 +81,16 @@ def _assert_same(got, ref, what=""):
     assert not bad.any(), f"{what}: {int(bad.sum())} of {bad.size} pixels differ, first at {np.argwhere(bad)[0]}"
 
 
-def _check(vwb, oracle, cost, left, right, search, kernel, path=None, what=""):
+def _check(vwb, oracle, cost, left, right, search, kernel, path=None, what="", trace=None, zone_int=False):
+    """parity with the oracle; with `trace`, also that the kernel the restated dispatch (tests/bm_reference.py) picks ran"""
     ref = oracle.calc_disparity(cost, left, right, search, kernel)
-    got = vwb.calc_disparity(cost, left, right, search, kernel)
+    run = lambda: vwb.calc_disparity(cost, left, right, search, kernel)
+    got = trace.run(run) if trace else run()
     _assert_same(got, ref, what)
     if path is not None:
         assert vwb.last_k1_stats()["path"] == path, what
+    if trace:
+        return trace.assert_hot(cost, left, right, search, kernel, zone_int)
 
 
 # ---- A: signed imagery with -0.0 ----------------------------------------------------------------------------------------
@@ -187,7 +193,7 @@ LIMITS = [  # id, cost, (W, H), search, kernel, lo, hi, texture, path
     ("abs-8192-k21", 0, (80, 60), (16, 8), (21, 21), -4096, 4096, "binary", FP64),
     # Sq: 4095^2 * 15 * 17 < 2^32 - 1 keeps K1 fast (window sums above 2^31); 15 x 19 goes to K1 screen; range 4096 to fp64
     ("sq-4095-k15x17", 1, (80, 48), (16, 8), (15, 17), 0, 4095, "binary", EXACT),
-    ("sq-4095-k15x19", 1, (80, 48), (16, 8), (15, 19), 0, 4095, "binary", EXACT),
+    ("sq-4095-k15x19", 1, (80, 48), (16, 8), (15, 19), 0, 4095, "binary", EXACT),      # K1 screen (asserted below)
     ("sq-4096-k15x17", 1, (80, 48), (16, 8), (15, 17), 0, 4096, "binary", FP64),
     # NCC on K1 screen: pixels in [0, 4095]
     ("ncc-vmax-4095", 2, (80, 48), (16, 8), (9, 9), 0, 4095, "uniform", EXACT),
@@ -206,10 +212,12 @@ LIMITS = [  # id, cost, (W, H), search, kernel, lo, hi, texture, path
 
 
 @pytest.mark.parametrize("case", LIMITS, ids=[c[0] for c in LIMITS])
-def test_b_range_limits(vwb, oracle, case):
+def test_b_range_limits(vwb, oracle, trace, case):
     what, cost, (W, H), search, kernel, lo, hi, texture, path = case
     left, right = make_pair(W, H, search, kernel, lo, hi, texture, seed=len(what) + W)
-    _check(vwb, oracle, cost, left, right, search, kernel, path, what)
+    exp = _check(vwb, oracle, cost, left, right, search, kernel, path, what, trace)
+    if what == "sq-4095-k15x19":                         # the kernel the comment above names
+        assert exp.family == "k1_screen_kernel"
 
 
 ZONE_LIMITS = [  # id, cost, K, lo, hi, texture
@@ -222,13 +230,18 @@ ZONE_LIMITS = [  # id, cost, K, lo, hi, texture
 
 
 @pytest.mark.parametrize("case", ZONE_LIMITS, ids=[c[0] for c in ZONE_LIMITS])
-def test_b5_zone_int_limits(vwb, oracle, monkeypatch, case):
+def test_b5_zone_int_limits(vwb, oracle, monkeypatch, trace, case):
     what, cost, k, lo, hi, texture = case
     left, right = make_pair(61, 45, (11, 9), (k, k), lo, hi, texture, seed=k + cost)
     monkeypatch.setenv("VWB200_K1_ZONE_INT", "1")
     n0 = vwb.kernel_launches()
-    _check(vwb, oracle, cost, left, right, (11, 9), (k, k), None, what)
+    exp = _check(vwb, oracle, cost, left, right, (11, 9), (k, k), None, what, trace, zone_int=True)
     assert vwb.kernel_launches() > n0
+    variant = what.rsplit("-", 1)[1]                       # the variant the id names
+    if variant in ("narrow", "wide"):
+        assert exp.family == "k1_zone_int_kernel" and exp.args[2] == (variant == "wide"), what
+    elif variant == "fp64":
+        assert exp.family == "k1_generic_kernel", what
 
 
 @pytest.mark.parametrize("cost", [0, 1, 2])

@@ -5,53 +5,8 @@ with the oracle bit for bit; this pins the oracle itself on inputs its known-ans
 import numpy as np
 import pytest
 
+from bm_reference import brute_calc_disparity
 from test_gpu_value_domain import make_pair
-
-
-def _box(a, kx, ky):
-    """kx x ky window sums by a summed-area table: exact for integer-valued a while the table stays below 2^53"""
-    c = np.zeros((a.shape[0] + 1, a.shape[1] + 1))
-    c[1:, 1:] = a.cumsum(0).cumsum(1)
-    return c[ky:, kx:] - c[:-ky, kx:] - c[ky:, :-kx] + c[:-ky, :-kx]
-
-
-def brute_calc_disparity(cost, left, right, search, kernel):
-    """best_of_search_convolution (Stereo/Correlation.cc:33-137): float32 per-pixel cost, float64 box sums, NCC as
-    S_lr * sqrt((1 / box(l^2)) * (1 / box(r^2))), strict '<' ('>' for NCC) over dy-major / dx-minor disparities,
-    best == worst -> invalid."""
-    l, r = np.asarray(left, np.float32), np.asarray(right, np.float32)
-    (sx, sy), (kx, ky) = search, kernel
-    H, W = l.shape[0] - ky + 1, l.shape[1] - kx + 1
-    r = r[:l.shape[0] + sy - 1, :l.shape[1] + sx - 1]
-    if cost == 2:
-        lp = 1.0 / _box((l * l).astype(np.float64), kx, ky)
-        rp = 1.0 / _box((r * r).astype(np.float64), kx, ky)
-    out = np.zeros((H, W, 3), np.int32)
-    out[..., 2] = 1
-    better = np.greater if cost == 2 else np.less
-    for dy in range(sy):
-        for dx in range(sx):
-            rs = r[dy:dy + l.shape[0], dx:dx + l.shape[1]]
-            if cost == 0:
-                c = np.abs(l - rs)
-            elif cost == 1:
-                d = l - rs
-                c = d * d
-            else:
-                c = l * rs
-            m = _box(c.astype(np.float64), kx, ky)
-            if cost == 2:
-                m = m * np.sqrt(lp * rp[dy:dy + H, dx:dx + W])
-            if dx == 0 and dy == 0:
-                best, worst = m.copy(), m.copy()
-                continue
-            up = better(m, best)
-            best[up] = m[up]
-            out[up, 0], out[up, 1] = dx, dy
-            down = ~up & ~better(m, worst)
-            worst[down] = m[down]
-    out[best == worst, 2] = 0
-    return out
 
 
 A1 = dict(lo=0, hi=2047, halves=True, negzero=True)
