@@ -125,6 +125,30 @@ int vwb200_parabola_subpixel(const float* disparity, int cols, int rows, const f
                              float* dest, ptrdiff_t dest_pitch, int on_device, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Disparity smoothing: vw::stereo::disparity_median_filter (src/vw/Stereo/Algorithms.cc:26-67), texture_measure
+ * (Algorithms.h:144-209) and texture_preserving_disparity_filter<float> (Algorithms.h:213-281).  Results are bit for bit
+ * the reference's (a zero may come out as -0.0 where the reference gives +0.0 or the reverse: its std::sort does not order
+ * them).  Disparities are cols x rows {dx, dy, valid} float triples, pitch in pixels; a pixel is valid when valid != 0.
+ *
+ * IN PLACE: the two disparity filters overwrite `disparity`.  The reference's `disparity_out = disparity_in` is ImageView's
+ * shallow copy, so there too the output shares the input's buffer, and each pixel's window sees the already filtered
+ * pixels above and to its left (raster order).  The engine computes exactly that order.  Processed pixels get valid = 1;
+ * every other pixel keeps all three floats.  The kernels take kernel_size / max_kernel_size up to 31 (VWB200_ENOIMPL
+ * above) and pitches up to INT_MAX / 93 pixels.  An in-place sweep that makes no progress for 10 s returns VWB200_ELOGIC
+ * ("wavefront stalled").
+ * ------------------------------------------------------------------------------------------- */
+/* kernel_size < 3: nothing changes.  Even sizes use the odd window below them (4 -> 3 x 3), as the reference does. */
+int vwb200_disparity_median_filter(float* disparity, int cols, int rows, ptrdiff_t pitch, int kernel_size, int on_device, void* stream);
+/* image: a plain float image (every pixel valid); out: cols x rows floats, row pitch opitch.  kernel_size < 1 ->
+ * VWB200_EARG (the reference leaves its output uninitialised there). */
+int vwb200_texture_measure(const float* image, int cols, int rows, ptrdiff_t pitch, int kernel_size, double gradient_weight,
+                           double stddev_weight, float* out, ptrdiff_t opitch, int on_device, void* stream);
+/* texture: cols x rows floats, row pitch tpitch.  max_kernel_size < 3 or texture_max <= 0: nothing changes.  A pixel whose
+ * texture gives a kernel above max_kernel_size is skipped silently (the reference prints a message to stdout there). */
+int vwb200_texture_preserving_disparity_filter(float* disparity, int cols, int rows, ptrdiff_t pitch, const float* texture,
+                                               ptrdiff_t tpitch, float texture_max, int max_kernel_size, int on_device, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * vw::stereo::calc_disparity_sgm (src/vw/Stereo/SGM.cc:167-230, SGM.h:361-376) ->
  * SemiGlobalMatcher::semi_global_matching_func (:2387-2448): u8_convert, (ternary) census costs for kernel 3/5/7/9,
  * per-pixel search boxes, SGM or MGM accumulation along 8 directions, integer winner with the reference's tie

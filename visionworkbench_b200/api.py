@@ -7,6 +7,8 @@ Names, argument order and error behaviour follow Vision Workbench:
   * pyramid_correlate         -- src/vw/Stereo/CorrelationView.h:195-230
   * cross_corr_consistency_check, rm_outliers_using_thresh, disparity_cleanup_using_thresh,
     disparity_mask            -- src/vw/Stereo/Correlate.h:52-58, DisparityMap.h:318-442,97-253
+  * disparity_median_filter, texture_measure, texture_preserving_disparity_filter
+                              -- src/vw/Stereo/Algorithms.cc:26-67, Algorithms.h:144-281
 
 There is no CPU path: every call goes to libvwb200.so (hand-written sm_90a kernels) and raises if
 the library or a CUDA device is missing.  Inputs may be numpy arrays (staged through HBM by the
@@ -109,6 +111,9 @@ def lib():
                                                    C.POINTER(I), C.POINTER(I), I, P]
         L.vwb200_sgm_disp_bounds.argtypes = [C.POINTER(SgmParams), P, I, I, Z, P, Z, P, I, I, Z, I, I, P, I, P]
         L.vwb200_parabola_subpixel.argtypes = [P, I, I, P, Z, P, I, I, Z, I, I, I, F, I, I, I, I, P, Z, I, P]
+        L.vwb200_disparity_median_filter.argtypes = [P, I, I, Z, I, I, P]
+        L.vwb200_texture_measure.argtypes = [P, I, I, Z, I, D, D, P, Z, I, P]
+        L.vwb200_texture_preserving_disparity_filter.argtypes = [P, I, I, Z, P, Z, F, I, I, P]
         L.vwb200_cross_corr_consistency_check.argtypes = [P, I, I, Z, P, I, I, Z, F, I, P]
         L.vwb200_rm_outliers_using_thresh.argtypes = [P, I, I, I, I, D, D, P, I, P]
         L.vwb200_disparity_cleanup_using_thresh.argtypes = [P, I, I, I, I, D, D, P, I, P]
@@ -359,6 +364,80 @@ def disparity_mask(disparity_map, left_mask, right_mask):
     _check(lib().vwb200_disparity_mask(a.ctypes.data, a.shape[1], a.shape[0], lm.ctypes.data, rm.ctypes.data,
                                        rm.shape[1], rm.shape[0], out.ctypes.data, 0, None))
     return out
+
+
+def _disparity_arg(disparity):
+    """(pointer, cols, rows, pitch in pixels, on_device) of a float32 (rows, cols, 3) disparity that is filtered in place"""
+    d = disparity
+    if _is_torch(d):
+        import torch
+        if not (d.is_cuda and d.dtype == torch.float32 and d.dim() == 3 and d.shape[2] == 3 and d.stride(2) == 1 and d.stride(1) == 3):
+            raise ArgumentErr("disparity must be a float32 CUDA tensor (rows, cols, 3) with dense pixels")
+        return d.data_ptr(), d.shape[1], d.shape[0], d.stride(0) // 3, 1
+    if not (isinstance(d, np.ndarray) and d.dtype == np.float32 and d.ndim == 3 and d.shape[2] == 3 and d.strides[2] == 4
+            and d.strides[1] == 12 and d.strides[0] % 12 == 0 and d.flags.writeable):
+        raise ArgumentErr("disparity must be a writeable float32 (rows, cols, 3) array with dense pixels (it is filtered in place)")
+    return d.ctypes.data, d.shape[1], d.shape[0], d.strides[0] // 12, 0
+
+
+def _image_arg(image, rows, cols, on_device):
+    """(keep-alive array, pointer, pitch in elements) of a float32 (rows, cols) image on the host or the device"""
+    if on_device:
+        import torch
+        if not (_is_torch(image) and image.is_cuda):
+            raise ArgumentErr("the texture image must be a CUDA tensor when the disparity is one")
+        t = image.float()
+        if t.stride(1) != 1:
+            t = t.contiguous()
+        if tuple(t.shape) != (rows, cols):
+            raise ArgumentErr("the texture image must have the disparity's size")
+        return t, t.data_ptr(), t.stride(0)
+    t = _np(image, np.float32)
+    if t.shape != (rows, cols):
+        raise ArgumentErr("the texture image must have the disparity's size")
+    return t, t.ctypes.data, t.shape[1]
+
+
+def disparity_median_filter(disparity, kernel_size):
+    """vw::stereo::disparity_median_filter (Stereo/Algorithms.cc:26-67).  Filters `disparity` (float32 (rows, cols, 3)
+    {dx, dy, valid}: a numpy array, or a CUDA tensor on the current stream) IN PLACE, in raster order, as the reference's
+    shallow `disparity_out = disparity_in` makes it do, and returns it."""
+    ptr, cols, rows, pitch, dev = _disparity_arg(disparity)
+    _check(lib().vwb200_disparity_median_filter(ptr, cols, rows, pitch, int(kernel_size), dev, _stream_ptr() if dev else None))
+    return disparity
+
+
+def texture_measure(image, kernel_size=9, gradient_weight=0.5, stddev_weight=0.5):
+    """vw::stereo::texture_measure (Stereo/Algorithms.h:144-209) of a float image (numpy, or a CUDA tensor on the current
+    stream): a new float32 image of the same size."""
+    if _is_torch(image):
+        import torch
+        t = image.float()
+        if t.dim() != 2 or t.stride(1) != 1:
+            t = t.contiguous()
+        out = torch.empty(t.shape, dtype=torch.float32, device=t.device)
+        _check(lib().vwb200_texture_measure(t.data_ptr(), t.shape[1], t.shape[0], t.stride(0), int(kernel_size), float(gradient_weight),
+                                            float(stddev_weight), out.data_ptr(), out.stride(0), 1, _stream_ptr()))
+        return out
+    a = _np(image, np.float32)
+    if a.ndim != 2:
+        raise ArgumentErr("texture_measure: the image must be 2-D")
+    out = np.empty_like(a)
+    _check(lib().vwb200_texture_measure(a.ctypes.data, a.shape[1], a.shape[0], a.shape[1], int(kernel_size), float(gradient_weight),
+                                        float(stddev_weight), out.ctypes.data, a.shape[1], 0, None))
+    return out
+
+
+def texture_preserving_disparity_filter(disparity, texture_image, texture_max=0.15, max_kernel_size=11):
+    """vw::stereo::texture_preserving_disparity_filter<float> (Stereo/Algorithms.h:213-281): smooths `disparity` (as in
+    disparity_median_filter: numpy or a CUDA tensor, filtered IN PLACE and returned) with a mean whose window shrinks as
+    the texture grows.  A pixel whose kernel would exceed max_kernel_size is skipped silently."""
+    ptr, cols, rows, pitch, dev = _disparity_arg(disparity)
+    keep, tptr, tpitch = _image_arg(texture_image, rows, cols, dev)
+    _check(lib().vwb200_texture_preserving_disparity_filter(ptr, cols, rows, pitch, tptr, tpitch, float(texture_max), int(max_kernel_size),
+                                                            dev, _stream_ptr() if dev else None))
+    del keep
+    return disparity
 
 
 class ParabolaSubpixelView:

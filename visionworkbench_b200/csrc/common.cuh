@@ -184,6 +184,15 @@ int log_region_launch(const float* g, int gw, int gx0, int gy0, int iw, int ih, 
 int parabola_launch(const float* disp, int cols, int bx0, int by0, int bw, int bh, const float* L, int lw, const float* R, int rw,
                     int srx0, int sry0, int kx, int ky, float* out, cudaStream_t st);
 
+// ---- disparity smoothing (k6_smoothing.cu) -----------------------------------------------------------
+static constexpr int kSmoothMaxKernel = 31;   // largest kernel_size / max_kernel_size the smoothing kernels take
+// in-place wavefront sweeps over W x H float disparity triples (pitch in pixels).  work: H + 2 ints of device scratch;
+// *err_host receives (asynchronously, on st) 1 when the sweep stalled
+int median_sweep_launch(float* d, int W, int H, ptrdiff_t pitch, int kernel_size, int* work, int* err_host, cudaStream_t st);
+int texture_filter_sweep_launch(float* d, int W, int H, ptrdiff_t pitch, const float* tex, ptrdiff_t tpitch, float texture_max,
+                                int max_kernel_size, int* work, int* err_host, cudaStream_t st);
+int texture_measure_launch(ImgF img, int kernel_size, double gw, double sw, float* out, ptrdiff_t opitch, cudaStream_t st);
+
 // ---- host-side restatement-free logic -----------------------------------------------------------
 struct Box { int x0, y0, x1, y1; };
 struct HostZone { Box img; Box disp; };

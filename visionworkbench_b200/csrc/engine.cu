@@ -9,6 +9,7 @@
 #include <chrono>
 #include "k5_sgm.cuh"
 #include <cstdarg>
+#include <climits>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -873,6 +874,40 @@ static int stage_in(const T* src, int w, int h, ptrdiff_t pitch, int on_device, 
 }
 
 
+// ---- disparity smoothing (Stereo/Algorithms.{h,cc}) ----------------------------------------------------------------
+// the two in-place filters: stage a host disparity through HBM, run the sweep, copy the result back, report a stall
+template <class Run>
+static int smoothing_in_place(const char* what, float* disparity, int cols, int rows, ptrdiff_t pitch, int on_device, void* stream,
+                              Run run) {
+  StreamGuard sg; VWB_TRY(sg.init(stream, on_device));
+  cudaStream_t st = sg.st;
+  int stalled = 0;
+  {
+    Arena ar(st);
+    float* d = disparity; ptrdiff_t dp = pitch;
+    int* work;
+    VWB_TRY(ar.alloc(&work, (size_t)rows + 2));
+    if (!on_device) {
+      VWB_TRY(ar.alloc(&d, (size_t)cols * rows * 3));
+      dp = cols;
+      VWB_CUDA(cudaMemcpy2DAsync(d, (size_t)cols * 12, disparity, (size_t)pitch * 12, (size_t)cols * 12, rows, cudaMemcpyHostToDevice, st));
+    }
+    VWB_TRY(run(d, dp, work, &stalled, st));
+    if (!on_device)
+      VWB_CUDA(cudaMemcpy2DAsync(disparity, (size_t)pitch * 12, d, (size_t)cols * 12, (size_t)cols * 12, rows, cudaMemcpyDeviceToHost, st));
+  }
+  VWB_CUDA(cudaStreamSynchronize(st));
+  if (stalled) { set_error("%s: wavefront stalled (a row waited more than 10 s for the row above)", what); return VWB200_ELOGIC; }
+  return VWB200_OK;
+}
+
+static int smoothing_check_disparity(const char* what, const float* disparity, int cols, int rows, ptrdiff_t pitch) {
+  if (!disparity) { set_error("%s: null pointer", what); return VWB200_EARG; }
+  if (cols < 0 || rows < 0 || pitch < cols) { set_error("%s: bad size %d x %d, pitch %td", what, cols, rows, pitch); return VWB200_EARG; }
+  if (pitch > INT_MAX / (3 * kSmoothMaxKernel)) { set_error("%s: pitch %td is above the supported %d", what, pitch, INT_MAX / (3 * kSmoothMaxKernel)); return VWB200_ENOIMPL; }
+  return VWB200_OK;
+}
+
 // ===================================================================================================
 // extern "C" ABI
 // ===================================================================================================
@@ -1310,6 +1345,60 @@ int vwb200_parabola_subpixel(const float* disparity, int cols, int rows, const f
     VWB_CUDA(cudaStreamSynchronize(st));
   }
   return VWB200_OK;
+}
+
+int vwb200_disparity_median_filter(float* disparity, int cols, int rows, ptrdiff_t pitch, int kernel_size, int on_device, void* stream) {
+  const char* what = "disparity_median_filter";
+  VWB_TRY(smoothing_check_disparity(what, disparity, cols, rows, pitch));
+  if (kernel_size > kSmoothMaxKernel) { set_error("%s: kernel_size %d is above the supported %d", what, kernel_size, kSmoothMaxKernel); return VWB200_ENOIMPL; }
+  VWB_TRY(ensure_device());
+  const int half = (kernel_size - 1) / 2;
+  if (kernel_size < 3 || cols <= 2 * half || rows <= 2 * half) return VWB200_OK;     // Algorithms.cc:34-35: nothing to filter
+  return smoothing_in_place(what, disparity, cols, rows, pitch, on_device, stream,
+                            [&](float* d, ptrdiff_t dp, int* work, int* err, cudaStream_t st) {
+                              return median_sweep_launch(d, cols, rows, dp, kernel_size, work, err, st);
+                            });
+}
+
+int vwb200_texture_measure(const float* image, int cols, int rows, ptrdiff_t pitch, int kernel_size, double gradient_weight,
+                           double stddev_weight, float* out, ptrdiff_t opitch, int on_device, void* stream) {
+  if (!image || !out) { set_error("texture_measure: null pointer"); return VWB200_EARG; }
+  if (cols < 0 || rows < 0 || pitch < cols || opitch < cols) { set_error("texture_measure: bad size %d x %d", cols, rows); return VWB200_EARG; }
+  if (kernel_size < 1) { set_error("texture_measure: kernel_size %d < 1", kernel_size); return VWB200_EARG; }
+  if (kernel_size > kSmoothMaxKernel) { set_error("texture_measure: kernel_size %d is above the supported %d", kernel_size, kSmoothMaxKernel); return VWB200_ENOIMPL; }
+  VWB_TRY(ensure_device());
+  if (!cols || !rows) return VWB200_OK;
+  StreamGuard sg; VWB_TRY(sg.init(stream, on_device));
+  cudaStream_t st = sg.st;
+  {
+    Arena ar(st);
+    const float* din; ptrdiff_t dp;
+    VWB_TRY(stage_in(image, cols, rows, pitch, on_device, ar, st, &din, &dp));
+    float* dout = out; ptrdiff_t dop = opitch;
+    if (!on_device) { VWB_TRY(ar.alloc(&dout, (size_t)cols * rows)); dop = cols; }
+    VWB_TRY(texture_measure_launch(ImgF{din, cols, rows, dp}, kernel_size, gradient_weight, stddev_weight, dout, dop, st));
+    if (!on_device)
+      VWB_CUDA(cudaMemcpy2DAsync(out, (size_t)opitch * 4, dout, (size_t)cols * 4, (size_t)cols * 4, rows, cudaMemcpyDeviceToHost, st));
+  }
+  VWB_CUDA(cudaStreamSynchronize(st));
+  return VWB200_OK;
+}
+
+int vwb200_texture_preserving_disparity_filter(float* disparity, int cols, int rows, ptrdiff_t pitch, const float* texture,
+                                               ptrdiff_t tpitch, float texture_max, int max_kernel_size, int on_device, void* stream) {
+  const char* what = "texture_preserving_disparity_filter";
+  VWB_TRY(smoothing_check_disparity(what, disparity, cols, rows, pitch));
+  if (!texture || tpitch < cols) { set_error("%s: bad texture image", what); return VWB200_EARG; }
+  if (max_kernel_size > kSmoothMaxKernel) { set_error("%s: max_kernel_size %d is above the supported %d", what, max_kernel_size, kSmoothMaxKernel); return VWB200_ENOIMPL; }
+  VWB_TRY(ensure_device());
+  if (max_kernel_size < 3 || texture_max <= 0 || !cols || !rows) return VWB200_OK;   // Algorithms.h:228-229
+  return smoothing_in_place(what, disparity, cols, rows, pitch, on_device, stream,
+                            [&](float* d, ptrdiff_t dp, int* work, int* err, cudaStream_t st) -> int {
+                              Arena ar(st);
+                              const float* t; ptrdiff_t tp;
+                              VWB_TRY(stage_in(texture, cols, rows, tpitch, on_device, ar, st, &t, &tp));
+                              return texture_filter_sweep_launch(d, cols, rows, dp, t, tp, texture_max, max_kernel_size, work, err, st);
+                            });
 }
 
 int vwb200_subsample_mask_by_two(const uint8_t* in, int w, int h, ptrdiff_t pitch, uint8_t* out, ptrdiff_t opitch, int on_device, void* stream) {
