@@ -166,6 +166,58 @@ def _np(a, dtype):
     return np.ascontiguousarray(a, dtype=dtype)
 
 
+def _ptr(x):
+    return x.data_ptr() if _is_torch(x) else x.ctypes.data
+
+
+def _raster(x, dtype, channels=1, on_device=None):
+    """(keep-alive, pointer, cols, rows, pitch in pixels, on_device) of an input raster (rows, cols[, channels]): a numpy array,
+    made C-contiguous `dtype`, or a torch CUDA tensor, converted to `dtype` and copied only when its rows are not dense.
+    on_device: where the call's other rasters are; a raster elsewhere is refused."""
+    if _is_torch(x):
+        import torch
+        t = x.to(getattr(torch, np.dtype(dtype).name))
+        if t.dim() < 2 or t.shape[0] == 0 or not t[0].is_contiguous() or t.stride(0) < t[0].numel():
+            t = t.contiguous()
+        r = (t, t.data_ptr(), t.shape[1], t.shape[0], t.stride(0) // channels, 1)
+    else:
+        a = _np(x, dtype)
+        r = (a, a.ctypes.data, a.shape[1], a.shape[0], a.shape[1], 0)
+    if on_device is not None and r[5] != on_device:
+        raise ArgumentErr("the inputs must all be numpy arrays or all be CUDA tensors")
+    return r
+
+
+def _optional(x, dtype):
+    """(keep-alive, pointer, cols, rows, pitch in pixels) of an optional host raster; (None, None, 0, 0, 0) without one"""
+    return (None, None, 0, 0, 0) if x is None else _raster(_np(x, dtype), dtype)[:5]
+
+
+def _output(beside, shape, dtype):
+    """an uninitialised output where `beside` lives: a CUDA tensor on its device, or a numpy array"""
+    if _is_torch(beside):
+        import torch
+        return torch.empty(shape, dtype=getattr(torch, np.dtype(dtype).name), device=beside.device)
+    return np.empty(shape, dtype)
+
+
+def _in_place(x, channels, what):
+    """(pointer, cols, rows, pitch in pixels, on_device) of a float32 (rows, cols, channels) raster the library writes
+    (a CUDA tensor, or a writeable numpy array) with dense pixels; ArgumentErr(what(on_device)) otherwise"""
+    if _is_torch(x):
+        import torch
+        ok = x.is_cuda and x.dtype == torch.float32 and x.dim() == 3 and x.shape[2] == channels and x.stride(2) == 1 and x.stride(1) == channels
+        r = (x.data_ptr(), x.shape[1], x.shape[0], x.stride(0) // channels, 1) if ok else None
+    else:
+        px = 4 * channels
+        ok = (isinstance(x, np.ndarray) and x.dtype == np.float32 and x.ndim == 3 and x.shape[2] == channels and x.strides[2] == 4
+              and x.strides[1] == px and x.strides[0] % px == 0 and x.flags.writeable)
+        r = (x.ctypes.data, x.shape[1], x.shape[0], x.strides[0] // px, 0) if ok else None
+    if not ok:
+        raise ArgumentErr(what(_is_torch(x)))
+    return r
+
+
 def calc_disparity(cost_type, left_in, right_in, search_volume, kernel_size):
     """vw::stereo::calc_disparity (Stereo/Correlation.h:50-57) on already-cropped rasters.
 
@@ -175,26 +227,14 @@ def calc_disparity(cost_type, left_in, right_in, search_volume, kernel_size):
     """
     sx, sy = search_volume
     kx, ky = kernel_size
-    if _is_torch(left_in):
-        import torch
-        l = left_in.contiguous().float()
-        r = right_in.contiguous().float()
-        H, W = l.shape[0] - ky + 1, l.shape[1] - kx + 1
-        if H <= 0 or W <= 0:
-            raise ArgumentErr("calc_disparity: Kernel size too large of active region.")
-        out = torch.empty((H, W, 3), dtype=torch.int32, device=l.device)
-        _check(lib().vwb200_calc_disparity(cost_type, l.data_ptr(), l.shape[1], l.shape[0], l.stride(0),
-                                           r.data_ptr(), r.shape[1], r.shape[0], r.stride(0),
-                                           sx, sy, kx, ky, out.data_ptr(), W, 1, _stream_ptr()))
-        return out
-    l, r = _np(left_in, np.float32), _np(right_in, np.float32)
-    H, W = l.shape[0] - ky + 1, l.shape[1] - kx + 1
+    l, lp, lw, lh, lpitch, dev = _raster(left_in, np.float32)
+    r, rp, rw, rh, rpitch, _ = _raster(right_in, np.float32, on_device=dev)
+    H, W = lh - ky + 1, lw - kx + 1
     if H <= 0 or W <= 0:
         raise ArgumentErr("calc_disparity: Kernel size too large of active region.")
-    out = np.empty((H, W, 3), np.int32)
-    _check(lib().vwb200_calc_disparity(cost_type, l.ctypes.data, l.shape[1], l.shape[0], l.shape[1],
-                                       r.ctypes.data, r.shape[1], r.shape[0], r.shape[1],
-                                       sx, sy, kx, ky, out.ctypes.data, W, 0, None))
+    out = _output(l, (H, W, 3), np.int32)
+    _check(lib().vwb200_calc_disparity(cost_type, lp, lw, lh, lpitch, rp, rw, rh, rpitch, sx, sy, kx, ky, _ptr(out), W, dev,
+                                       _stream_ptr() if dev else None))
     return out
 
 
@@ -205,22 +245,13 @@ def calc_disparity_sgm(left_in, right_in, search_volume, kernel_size, p1=0, p2=0
     cannot cover are cropped)."""
     sx, sy = search_volume
     ow, oh = C.c_int(0), C.c_int(0)
-    if _is_torch(left_in):
-        import torch
-        l = left_in.contiguous().float()
-        r = right_in.contiguous().float()
-        _check(lib().vwb200_sgm_calc_disparity(l.data_ptr(), l.shape[1], l.shape[0], l.stride(0), r.data_ptr(), r.shape[1], r.shape[0], r.stride(0),
-                                               sx, sy, kernel_size, p1, p2, None, 0, C.byref(ow), C.byref(oh), 1, None))
-        out = torch.empty((max(oh.value, 0), max(ow.value, 0), 3), dtype=torch.int32, device=l.device)
-        _check(lib().vwb200_sgm_calc_disparity(l.data_ptr(), l.shape[1], l.shape[0], l.stride(0), r.data_ptr(), r.shape[1], r.shape[0], r.stride(0),
-                                               sx, sy, kernel_size, p1, p2, out.data_ptr(), ow.value, C.byref(ow), C.byref(oh), 1, _stream_ptr()))
-        return out
-    l, r = _np(left_in, np.float32), _np(right_in, np.float32)
-    args = (l.ctypes.data, l.shape[1], l.shape[0], l.shape[1], r.ctypes.data, r.shape[1], r.shape[0], r.shape[1], sx, sy, kernel_size, p1, p2)
-    _check(lib().vwb200_sgm_calc_disparity(*args, None, 0, C.byref(ow), C.byref(oh), 0, None))
-    out = np.empty((max(oh.value, 0), max(ow.value, 0), 3), np.int32)
-    if out.size:
-        _check(lib().vwb200_sgm_calc_disparity(*args, out.ctypes.data, ow.value, C.byref(ow), C.byref(oh), 0, None))
+    l, lp, lw, lh, lpitch, dev = _raster(left_in, np.float32)
+    r, rp, rw, rh, rpitch, _ = _raster(right_in, np.float32, on_device=dev)
+    args = (lp, lw, lh, lpitch, rp, rw, rh, rpitch, sx, sy, kernel_size, p1, p2)
+    _check(lib().vwb200_sgm_calc_disparity(*args, None, 0, C.byref(ow), C.byref(oh), dev, None))
+    out = _output(l, (max(oh.value, 0), max(ow.value, 0), 3), np.int32)
+    if ow.value > 0 and oh.value > 0:
+        _check(lib().vwb200_sgm_calc_disparity(*args, _ptr(out), ow.value, C.byref(ow), C.byref(oh), dev, _stream_ptr() if dev else None))
     return out
 
 
@@ -265,20 +296,14 @@ def calc_disparity_sgm_ex(cost_type, left_in, right_in, search_volume, kernel_si
     sub = np.zeros((h, w, 3), np.float32)
     bo = np.zeros((h, w, 4), np.int32)
     if out.size:
-        lm = _np(left_mask, np.uint8) if left_mask is not None else None
-        rm = _np(right_mask, np.uint8) if right_mask is not None else None
-        pv = _np(prev_disparity, np.int32) if prev_disparity is not None else None
-        bd = _np(bounds, np.int32) if bounds is not None else None
-        if lm is not None and lm.shape != (h, w):
+        lm, rm, pv, bd = _optional(left_mask, np.uint8), _optional(right_mask, np.uint8), _optional(prev_disparity, np.int32), \
+            _optional(bounds, np.int32)
+        if lm[0] is not None and lm[0].shape != (h, w):
             raise LogicErr("Left mask size does not match the output size.")
-        if bd is not None and bd.shape != (h, w, 4):
+        if bd[0] is not None and bd[0].shape != (h, w, 4):
             raise ArgumentErr("sgm: bounds must be (out_h, out_w, 4)")
-        _check(lib().vwb200_sgm_calc_disparity_ex(
-            *head, lm.ctypes.data if lm is not None else None, w, rm.ctypes.data if rm is not None else None,
-            rm.shape[1] if rm is not None else 0, rm.shape[0] if rm is not None else 0, rm.shape[1] if rm is not None else 0,
-            pv.ctypes.data if pv is not None else None, pv.shape[1] if pv is not None else 0, pv.shape[0] if pv is not None else 0,
-            pv.shape[1] if pv is not None else 0, bd.ctypes.data if bd is not None else None,
-            out.ctypes.data, w, sub.ctypes.data, w, bo.ctypes.data if return_bounds else None, C.byref(ow), C.byref(oh), 0, None))
+        _check(lib().vwb200_sgm_calc_disparity_ex(*head, lm[1], w, *rm[1:], *pv[1:], bd[1], out.ctypes.data, w, sub.ctypes.data, w,
+                                                  bo.ctypes.data if return_bounds else None, C.byref(ow), C.byref(oh), 0, None))
     return (out, sub, bo) if return_bounds else (out, sub)
 
 
@@ -289,16 +314,11 @@ def sgm_disp_bounds(shape, search_volume, search_buffer=(2, 2), prev_disparity=N
     h, w = int(shape[0]), int(shape[1])
     sp = _sgm_params(search_volume, 5, CENSUS_TRANSFORM, use_mgm, 0, search_buffer, memory_limit_mb, conserve_level=conserve_level,
                      assumed_threads=assumed_threads)
-    lm = _np(left_mask, np.uint8) if left_mask is not None else None
-    rm = _np(right_mask, np.uint8) if right_mask is not None else None
-    pv = _np(prev_disparity, np.int32) if prev_disparity is not None else None
-    if lm is not None and lm.shape != (h, w):
+    lm, rm, pv = _optional(left_mask, np.uint8), _optional(right_mask, np.uint8), _optional(prev_disparity, np.int32)
+    if lm[0] is not None and lm[0].shape != (h, w):
         raise LogicErr("Left mask size does not match the output size.")
     out = np.zeros((h, w, 4), np.int32)
-    _check(lib().vwb200_sgm_disp_bounds(
-        C.byref(sp), pv.ctypes.data if pv is not None else None, pv.shape[1] if pv is not None else 0, pv.shape[0] if pv is not None else 0,
-        pv.shape[1] if pv is not None else 0, lm.ctypes.data if lm is not None else None, w, rm.ctypes.data if rm is not None else None,
-        rm.shape[1] if rm is not None else 0, rm.shape[0] if rm is not None else 0, rm.shape[1] if rm is not None else 0, w, h, out.ctypes.data, 0, None))
+    _check(lib().vwb200_sgm_disp_bounds(C.byref(sp), *pv[1:], lm[1], w, *rm[1:], w, h, out.ctypes.data, 0, None))
     return out
 
 
@@ -368,34 +388,8 @@ def disparity_mask(disparity_map, left_mask, right_mask):
 
 def _disparity_arg(disparity):
     """(pointer, cols, rows, pitch in pixels, on_device) of a float32 (rows, cols, 3) disparity that is filtered in place"""
-    d = disparity
-    if _is_torch(d):
-        import torch
-        if not (d.is_cuda and d.dtype == torch.float32 and d.dim() == 3 and d.shape[2] == 3 and d.stride(2) == 1 and d.stride(1) == 3):
-            raise ArgumentErr("disparity must be a float32 CUDA tensor (rows, cols, 3) with dense pixels")
-        return d.data_ptr(), d.shape[1], d.shape[0], d.stride(0) // 3, 1
-    if not (isinstance(d, np.ndarray) and d.dtype == np.float32 and d.ndim == 3 and d.shape[2] == 3 and d.strides[2] == 4
-            and d.strides[1] == 12 and d.strides[0] % 12 == 0 and d.flags.writeable):
-        raise ArgumentErr("disparity must be a writeable float32 (rows, cols, 3) array with dense pixels (it is filtered in place)")
-    return d.ctypes.data, d.shape[1], d.shape[0], d.strides[0] // 12, 0
-
-
-def _image_arg(image, rows, cols, on_device):
-    """(keep-alive array, pointer, pitch in elements) of a float32 (rows, cols) image on the host or the device"""
-    if on_device:
-        import torch
-        if not (_is_torch(image) and image.is_cuda):
-            raise ArgumentErr("the texture image must be a CUDA tensor when the disparity is one")
-        t = image.float()
-        if t.stride(1) != 1:
-            t = t.contiguous()
-        if tuple(t.shape) != (rows, cols):
-            raise ArgumentErr("the texture image must have the disparity's size")
-        return t, t.data_ptr(), t.stride(0)
-    t = _np(image, np.float32)
-    if t.shape != (rows, cols):
-        raise ArgumentErr("the texture image must have the disparity's size")
-    return t, t.ctypes.data, t.shape[1]
+    return _in_place(disparity, 3, lambda dev: "disparity must be a float32 CUDA tensor (rows, cols, 3) with dense pixels" if dev else
+                     "disparity must be a writeable float32 (rows, cols, 3) array with dense pixels (it is filtered in place)")
 
 
 def disparity_median_filter(disparity, kernel_size):
@@ -410,21 +404,12 @@ def disparity_median_filter(disparity, kernel_size):
 def texture_measure(image, kernel_size=9, gradient_weight=0.5, stddev_weight=0.5):
     """vw::stereo::texture_measure (Stereo/Algorithms.h:144-209) of a float image (numpy, or a CUDA tensor on the current
     stream): a new float32 image of the same size."""
-    if _is_torch(image):
-        import torch
-        t = image.float()
-        if t.dim() != 2 or t.stride(1) != 1:
-            t = t.contiguous()
-        out = torch.empty(t.shape, dtype=torch.float32, device=t.device)
-        _check(lib().vwb200_texture_measure(t.data_ptr(), t.shape[1], t.shape[0], t.stride(0), int(kernel_size), float(gradient_weight),
-                                            float(stddev_weight), out.data_ptr(), out.stride(0), 1, _stream_ptr()))
-        return out
-    a = _np(image, np.float32)
-    if a.ndim != 2:
+    if not _is_torch(image) and _np(image, np.float32).ndim != 2:
         raise ArgumentErr("texture_measure: the image must be 2-D")
-    out = np.empty_like(a)
-    _check(lib().vwb200_texture_measure(a.ctypes.data, a.shape[1], a.shape[0], a.shape[1], int(kernel_size), float(gradient_weight),
-                                        float(stddev_weight), out.ctypes.data, a.shape[1], 0, None))
+    t, ptr, cols, rows, pitch, dev = _raster(image, np.float32)
+    out = _output(t, t.shape, np.float32)
+    _check(lib().vwb200_texture_measure(ptr, cols, rows, pitch, int(kernel_size), float(gradient_weight), float(stddev_weight), _ptr(out),
+                                        cols, dev, _stream_ptr() if dev else None))
     return out
 
 
@@ -433,10 +418,13 @@ def texture_preserving_disparity_filter(disparity, texture_image, texture_max=0.
     disparity_median_filter: numpy or a CUDA tensor, filtered IN PLACE and returned) with a mean whose window shrinks as
     the texture grows.  A pixel whose kernel would exceed max_kernel_size is skipped silently."""
     ptr, cols, rows, pitch, dev = _disparity_arg(disparity)
-    keep, tptr, tpitch = _image_arg(texture_image, rows, cols, dev)
+    if dev and not (_is_torch(texture_image) and texture_image.is_cuda):
+        raise ArgumentErr("the texture image must be a CUDA tensor when the disparity is one")
+    keep, tptr, tcols, trows, tpitch, _ = _raster(texture_image if dev else _np(texture_image, np.float32), np.float32)
+    if tuple(keep.shape) != (rows, cols):
+        raise ArgumentErr("the texture image must have the disparity's size")
     _check(lib().vwb200_texture_preserving_disparity_filter(ptr, cols, rows, pitch, tptr, tpitch, float(texture_max), int(max_kernel_size),
                                                             dev, _stream_ptr() if dev else None))
-    del keep
     return disparity
 
 
@@ -530,41 +518,21 @@ class PyramidCorrelationView:
                              int(region_ul[0]), int(region_ul[1]), int(bool(write_debug_images)), int(sgm_threads), float(memory_limit_mb))
         self._h = C.c_void_p()
         _check(lib().vwb200_corr_create(C.byref(self._p), C.byref(self._h)))
-        self._diff = None
+        self._diff = lr_disp_diff
         if lr_disp_diff is not None:
-            if _is_torch(lr_disp_diff):
-                d = lr_disp_diff
-                assert d.dtype.is_floating_point and d.element_size() == 4 and d.dim() == 3 and d.shape[2] == 2 and d.stride(2) == 1 and d.stride(1) == 2
-                _check(lib().vwb200_corr_set_lr_disp_diff(self._h, d.data_ptr(), d.shape[1], d.shape[0], d.stride(0) // 2, 1))
-            else:
-                d = lr_disp_diff
-                if not (isinstance(d, np.ndarray) and d.dtype == np.float32 and d.ndim == 3 and d.shape[2] == 2 and d.strides[2] == 4 and d.strides[1] == 8):
-                    raise ArgumentErr("lr_disp_diff must be a float32 (rows, cols, 2) array")
-                _check(lib().vwb200_corr_set_lr_disp_diff(self._h, d.ctypes.data, d.shape[1], d.shape[0], d.strides[0] // 8, 0))
-            self._diff = d
-        self._keep = None
+            ptr, cols, rows, pitch, dev = _in_place(lr_disp_diff, 2, lambda dev: "lr_disp_diff must be a float32 (rows, cols, 2) array")
+            _check(lib().vwb200_corr_set_lr_disp_diff(self._h, ptr, cols, rows, pitch, dev))
         self._device = _is_torch(left)
         if self._device:
             import torch
-            l, r = left.contiguous().float(), right.contiguous().float()
-            if tuple(left_mask.shape) != tuple(l.shape) or tuple(right_mask.shape) != tuple(r.shape):
-                raise ArgumentErr("masks must have the size of their images")
-            lm = (left_mask != 0).to(torch.uint8).contiguous() if left_mask.dtype != torch.uint8 else left_mask.contiguous()
-            rm = (right_mask != 0).to(torch.uint8).contiguous() if right_mask.dtype != torch.uint8 else right_mask.contiguous()
-            self._keep = (l, r, lm, rm)
-            _check(lib().vwb200_corr_set_inputs(self._h, l.data_ptr(), l.shape[1], l.shape[0], l.stride(0),
-                                                r.data_ptr(), r.shape[1], r.shape[0], r.stride(0),
-                                                lm.data_ptr(), lm.stride(0), rm.data_ptr(), rm.stride(0), 1))
-        else:
-            l, r = _np(left, np.float32), _np(right, np.float32)
-            lm, rm = _np(left_mask, np.uint8), _np(right_mask, np.uint8)
-            if lm.shape != l.shape or rm.shape != r.shape:
-                raise ArgumentErr("masks must have the size of their images")
-            if streamed:          # the rasters stay on the host; each rasterize() uploads its tile's region of interest
-                self._keep = (l, r, lm, rm)
-            _check(lib().vwb200_corr_set_inputs(self._h, l.ctypes.data, l.shape[1], l.shape[0], l.shape[1],
-                                                r.ctypes.data, r.shape[1], r.shape[0], r.shape[1],
-                                                lm.ctypes.data, lm.shape[1], rm.ctypes.data, rm.shape[1], 2 if streamed else 0))
+            left_mask, right_mask = [m if m.dtype == torch.uint8 else m != 0 for m in (left_mask, right_mask)]
+        l = _raster(left, np.float32)
+        r, lm, rm = _raster(right, np.float32, on_device=l[5]), _raster(left_mask, np.uint8, on_device=l[5]), _raster(right_mask, np.uint8, on_device=l[5])
+        if tuple(lm[0].shape) != tuple(l[0].shape) or tuple(rm[0].shape) != tuple(r[0].shape):
+            raise ArgumentErr("masks must have the size of their images")
+        # the library copies host rasters into HBM, except streamed ones: each rasterize() uploads its tile's region of interest
+        self._keep = tuple(x[0] for x in (l, r, lm, rm)) if self._device or streamed else None
+        _check(lib().vwb200_corr_set_inputs(self._h, *l[1:5], *r[1:5], lm[1], lm[4], rm[1], rm[4], 1 if self._device else 2 if streamed else 0))
 
     def __del__(self):
         try:
@@ -599,17 +567,11 @@ class PyramidCorrelationView:
     def _run(self, fn, dest, bbox):
         b = _bbox(bbox) if bbox is not None else (0, 0, self.cols(), self.rows())
         w, h = b[2] - b[0], b[3] - b[1]
-        if dest is not None and _is_torch(dest) or (dest is None and self._device):
-            import torch
-            if dest is None:
-                dest = torch.empty((h, w, 3), dtype=torch.float32, device=self._keep[0].device)
-            assert dest.shape == (h, w, 3) and dest.dtype == torch.float32 and dest.stride(2) == 1 and dest.stride(1) == 3
-            _check(fn(self._h, b[0], b[1], b[2], b[3], dest.data_ptr(), dest.stride(0) // 3, 1, _stream_ptr()))
-            return dest
         if dest is None:
-            dest = np.empty((h, w, 3), np.float32)
-        assert dest.shape == (h, w, 3) and dest.dtype == np.float32 and dest.strides[2] == 4 and dest.strides[1] == 12
-        _check(fn(self._h, b[0], b[1], b[2], b[3], dest.ctypes.data, dest.strides[0] // 12, 0, None))
+            dest = _output(self._keep[0] if self._device else None, (h, w, 3), np.float32)
+        assert tuple(dest.shape) == (h, w, 3)
+        ptr, _, _, pitch, dev = _in_place(dest, 3, lambda dev: "dest must be a float32 (h, w, 3) raster with dense pixels")
+        _check(fn(self._h, b[0], b[1], b[2], b[3], ptr, pitch, dev, _stream_ptr() if dev else None))
         return dest
 
     def prerasterize(self, bbox):

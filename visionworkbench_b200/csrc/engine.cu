@@ -444,6 +444,38 @@ static int filtered_region(ImgF img, int mode, float width, Box reg, float** out
   return log_region_launch(g, ew, big.x0, big.y0, img.w, img.h, reg.x0, reg.y0, w, h, o, st);
 }
 
+// The outlier filter chain (CorrelationView.cc:713-744): pass 1 of rm_outliers_using_thresh, either unpadded or padded and
+// followed by pass 2 (disparity_cleanup_using_thresh), then disparity_mask when masks are given.  in -> out, w x h, dense;
+// out may be in when there are masks.
+static int outlier_filter_chain(const vwb200_dispi* in, int w, int h, int hx, int hy, double pt, double rt, bool cleanup, ImgB lmask,
+                                ImgB rmask, vwb200_dispi* out, Arena& ar, cudaStream_t st) {
+  vwb200_dispi *t1, *t2 = out;
+  if (lmask.p) VWB_TRY(ar.alloc(&t2, (size_t)w * h));
+  if (cleanup) {
+    VWB_TRY(ar.alloc(&t1, (size_t)(w + 2) * (h + 2)));
+    VWB_TRY(rm_outliers_launch(in, w, h, hx, hy, pt, rt, -1, -1, w + 2, h + 2, t1, st));
+    VWB_TRY(cleanup_pass2_launch(t1, w, h, t2, st));
+  } else {
+    VWB_TRY(rm_outliers_launch(in, w, h, hx, hy, pt, rt, 0, 0, w, h, t2, st));
+  }
+  if (lmask.p) VWB_TRY(disparity_mask_launch(t2, w, h, lmask, rmask, out, st));
+  return VWB200_OK;
+}
+
+// calc_disparity_sgm's memory limit and assumed thread count when a caller passes none (SGM.cc:715-716)
+static constexpr double kSgmMemoryLimitMb = 6000.0;
+static constexpr int kSgmThreads = 4;
+static SgmArgs sgm_args(const vwb200_sgm_params& sp) {
+  SgmArgs a;
+  a.sx = sp.search_x; a.sy = sp.search_y; a.k = sp.kernel_size;
+  a.ternary = sp.cost_type == VWB200_TERNARY_CENSUS_TRANSFORM; a.ternary_threshold = sp.ternary_threshold;
+  a.p1 = sp.p1; a.p2 = sp.p2; a.use_mgm = sp.use_mgm; a.subpixel_mode = sp.subpixel_mode;
+  a.buf_x = sp.search_buffer_x; a.buf_y = sp.search_buffer_y; a.conserve_level = sp.conserve_level;
+  a.memory_limit_mb = sp.memory_limit_mb > 0 ? sp.memory_limit_mb : kSgmMemoryLimitMb;
+  a.assumed_threads = sp.assumed_threads > 0 ? sp.assumed_threads : kSgmThreads;
+  return a;
+}
+
 // ---------------------------------------------------------------------------------------------------
 // the view handle
 // ---------------------------------------------------------------------------------------------------
@@ -477,7 +509,7 @@ struct vwb200_corr {
   }
   // optional lr_disp_diff output (CorrelationView.h:67-68): PixelMask<float> pairs, caller-owned
   float* diff = nullptr; int diff_cols = 0, diff_rows = 0; ptrdiff_t diff_pitch = 0; int diff_on_device = 0;
-  struct DiffTile { float* d = nullptr; ptrdiff_t pitch = 0; int ox = 0, oy = 0; };   // device view of the processed box's window
+  struct DiffTile { float* d = nullptr; ptrdiff_t pitch = 0; };   // device view of the processed box's window
   int prerasterize(Box bbox, vwb200_dispi** d_disp_out, float** d_sub_out, int* all_invalid, const DiffTile& df, Arena& ar, cudaStream_t st) const;
   int prerasterize_sgm(Box bbox, const std::vector<struct LevelImgsT>& py, int levels, vwb200_dispi** d_disp_out, float** d_sub_out,
                        const DiffTile& df, Arena& ar, cudaStream_t st) const;
@@ -693,21 +725,11 @@ int vwb200_corr::prerasterize(Box bbox, vwb200_dispi** d_disp_out, float** d_sub
       VWB_TRY(ar.alloc(&d_post, post.size()));
       VWB_CUDA(cudaMemcpyAsync(d_post, post.data(), post.size() * sizeof(int2), cudaMemcpyHostToDevice, st));
       VWB_TRY(zone_post_launch(d_tl, ntl, d_zl, d_zr, d_post, disp, rl, p.consistency_threshold, tile_w, tile_h, st,
-                               (level == 0 && check) ? df.d : nullptr, df.pitch, df.ox, df.oy));
+                               (level == 0 && check) ? df.d : nullptr, df.pitch));
     }
-    if (p.filter_half_kernel > 0) {   // :713-744
-      const int fh = p.filter_half_kernel;
-      vwb200_dispi *t1, *t2;
-      VWB_TRY(ar.alloc(&t2, (size_t)dw * dh));
-      if (level != 0) {
-        VWB_TRY(ar.alloc(&t1, (size_t)(dw + 2) * (dh + 2)));
-        VWB_TRY(rm_outliers_launch(disp, dw, dh, fh, fh, 3.0, 0.5, -1, -1, dw + 2, dh + 2, t1, st));
-        VWB_TRY(cleanup_pass2_launch(t1, dw, dh, t2, st));
-      } else {
-        VWB_TRY(rm_outliers_launch(disp, dw, dh, fh, fh, 3.0, 0.5, 0, 0, dw, dh, t2, st));
-      }
-      VWB_TRY(disparity_mask_launch(t2, dw, dh, ImgB{lv.lm, lv.lmw, lv.lmh, lv.lmw}, ImgB{lv.rm, lv.rmw, lv.rmh, lv.rmw}, disp, st));
-    }
+    if (p.filter_half_kernel > 0)   // :713-744
+      VWB_TRY(outlier_filter_chain(disp, dw, dh, p.filter_half_kernel, p.filter_half_kernel, 3.0, 0.5, level != 0,
+                                   ImgB{lv.lm, lv.lmw, lv.lmh, lv.lmw}, ImgB{lv.rm, lv.rmw, lv.rmh, lv.rmw}, disp, ar, st));
     if (p.blob_filter_area / scaling >= 1) {   // :746-749, disparity_blob_filter (:242-271)
       int* work;
       VWB_TRY(ar.alloc(&work, (size_t)2 * dw * dh));
@@ -739,7 +761,7 @@ int vwb200_corr::prerasterize(Box bbox, vwb200_dispi** d_disp_out, float** d_sub
   }
   const LevelImgs& l0 = py[0];
   if (l0.lmw != bw || l0.lmh != bh) { set_error("PyramidCorrelation: Solved disparity doesn't match requested bbox size."); return VWB200_EMATH; }
-  if (df.d) VWB_TRY(diff_invalidate_launch(disp, bw, bh, df.d, df.pitch, df.ox, df.oy, st));   // :848-857
+  if (df.d) VWB_TRY(diff_invalidate_launch(disp, bw, bh, df.d, df.pitch, 0, 0, st));   // :848-857
   if (prof) {
     const double enq = ms_since(t_loop);
     cudaStreamSynchronize(st);
@@ -786,8 +808,8 @@ int vwb200_corr::prerasterize_sgm(Box bbox, const std::vector<LevelImgs>& py, in
     a.ternary = p.cost_type == VWB200_TERNARY_CENSUS_TRANSFORM; a.ternary_threshold = 5;
     a.use_mgm = use_mgm; a.subpixel_mode = p.sgm_subpixel_mode;
     a.buf_x = p.sgm_search_buffer_x; a.buf_y = p.sgm_search_buffer_y;
-    a.memory_limit_mb = p.memory_limit_mb > 0 ? p.memory_limit_mb : 6000.0;
-    a.assumed_threads = p.sgm_threads > 0 ? p.sgm_threads : 4;
+    a.memory_limit_mb = p.memory_limit_mb > 0 ? p.memory_limit_mb : kSgmMemoryLimitMb;
+    a.assumed_threads = p.sgm_threads > 0 ? p.sgm_threads : kSgmThreads;
     a.lmask = ImgB{lv.lm, lv.lmw, lv.lmh, lv.lmw}; a.rmask = ImgB{lv.rm, lv.rmw, lv.rmh, lv.rmw};
     if (level < levels) { a.prev = prev; a.pw = pw; a.ph = ph; a.ppitch = pw; }
     int ow = 0, oh = 0;
@@ -825,28 +847,15 @@ int vwb200_corr::prerasterize_sgm(Box bbox, const std::vector<LevelImgs>& py, in
       VWB_TRY(sgm_run(b, ar, st));
       // the R->L disparity enters the check shifted by -size and goes on un-shifted (:548-549, 586)
       VWB_TRY(consistency_launch(disp, dw, dh, dw, disp_rl, rlw, rlh, rlw, p.consistency_threshold, st, -dsx, -dsy,
-                                 level == 0 ? df.d : nullptr, df.pitch, df.ox, df.oy));
+                                 level == 0 ? df.d : nullptr, df.pitch));
     }
     if (p.filter_half_kernel > 0) {                                                             // :713-744
       const int fh = p.filter_half_kernel;
-      vwb200_dispi *t1, *t2;
-      VWB_TRY(ar.alloc(&t2, (size_t)dw * dh));
-      if (level != 0) {
-        VWB_TRY(ar.alloc(&t1, (size_t)(dw + 2) * (dh + 2)));
-        VWB_TRY(rm_outliers_launch(disp, dw, dh, fh, fh, 3.0, 0.5, -1, -1, dw + 2, dh + 2, t1, st));
-        VWB_TRY(cleanup_pass2_launch(t1, dw, dh, t2, st));
-      } else {
-        VWB_TRY(rm_outliers_launch(disp, dw, dh, fh, fh, 3.0, 0.5, 0, 0, dw, dh, t2, st));
-      }
-      VWB_TRY(disparity_mask_launch(t2, dw, dh, ImgB{lv.lm, lv.lmw, lv.lmh, lv.lmw}, ImgB{lv.rm, lv.rmw, lv.rmh, lv.rmw}, disp, st));
-      if (level != 0 && check_rl) {
-        vwb200_dispi *u1, *u2;
-        VWB_TRY(ar.alloc(&u1, (size_t)(rlw + 2) * (rlh + 2)));
-        VWB_TRY(ar.alloc(&u2, (size_t)rlw * rlh));
-        VWB_TRY(rm_outliers_launch(disp_rl, rlw, rlh, fh, fh, 3.0, 0.5, -1, -1, rlw + 2, rlh + 2, u1, st));
-        VWB_TRY(cleanup_pass2_launch(u1, rlw, rlh, u2, st));
-        VWB_TRY(disparity_mask_launch(u2, rlw, rlh, ImgB{rrm, rlw, rlh, rlw}, ImgB{lrm, lrmw, lrmh, lrmw}, disp_rl, st));
-      }
+      VWB_TRY(outlier_filter_chain(disp, dw, dh, fh, fh, 3.0, 0.5, level != 0, ImgB{lv.lm, lv.lmw, lv.lmh, lv.lmw},
+                                   ImgB{lv.rm, lv.rmw, lv.rmh, lv.rmw}, disp, ar, st));
+      if (level != 0 && check_rl)
+        VWB_TRY(outlier_filter_chain(disp_rl, rlw, rlh, fh, fh, 3.0, 0.5, true, ImgB{rrm, rlw, rlh, rlw}, ImgB{lrm, lrmw, lrmh, lrmw},
+                                     disp_rl, ar, st));
     }
     const int area = p.blob_filter_area / scaling;                                               // :747-749
     if (area >= 1) {
@@ -857,46 +866,72 @@ int vwb200_corr::prerasterize_sgm(Box bbox, const std::vector<LevelImgs>& py, in
     }
   }
   if (dw != bw || dh != bh) { set_error("PyramidCorrelation: Solved disparity doesn't match requested bbox size."); return VWB200_EMATH; }
-  if (df.d) VWB_TRY(diff_invalidate_launch(disp, bw, bh, df.d, df.pitch, df.ox, df.oy, st));
+  if (df.d) VWB_TRY(diff_invalidate_launch(disp, bw, bh, df.d, df.pitch, 0, 0, st));
   *d_disp_out = disp; *d_sub_out = sub;
   return VWB200_OK;
 }
 
-// stage a host image into HBM (or pass a device image through)
-template <class T>
-static int stage_in(const T* src, int w, int h, ptrdiff_t pitch, int on_device, Arena& ar, cudaStream_t st, const T** out, ptrdiff_t* opitch) {
-  if (on_device) { *out = src; *opitch = pitch; return VWB200_OK; }
-  T* d;
-  VWB_TRY(ar.alloc(&d, (size_t)w * h));
-  VWB_CUDA(cudaMemcpy2DAsync(d, (size_t)w * sizeof(T), src, (size_t)pitch * sizeof(T), (size_t)w * sizeof(T), h, cudaMemcpyHostToDevice, st));
-  *out = d; *opitch = w;
-  return VWB200_OK;
-}
+// One call of the C ABI: its stream, its stream-ordered scratch, and the moves of the caller's rasters between the host and
+// HBM.  Widths and pitches count elements of T (a float triple is 3 floats, a search box 4 int32).  finish() copies the
+// staged outputs back and synchronises the stream: every call returns with its work done, device-resident calls included.
+struct AbiCall {
+  StreamGuard sg;
+  Arena ar{nullptr};
+  cudaStream_t st = nullptr;
+  struct CopyBack { void* dst; size_t dpitch; const void* src; size_t row; int h; cudaMemcpyKind kind; const int* unless; };
+  std::vector<CopyBack> backs;
 
+  int open(void* stream, int device_resident) {
+    VWB_TRY(sg.init(stream, device_resident));
+    st = ar.st = sg.st;
+    return VWB200_OK;
+  }
+  // an input: the caller's device raster, or a dense HBM copy of the host raster
+  template <class T> int in(const T* src, int w, int h, ptrdiff_t pitch, int on_device, const T** dev, ptrdiff_t* dpitch) {
+    if (on_device) { *dev = src; *dpitch = pitch; return VWB200_OK; }
+    T* d;
+    VWB_TRY(ar.alloc(&d, (size_t)w * h));
+    VWB_CUDA(cudaMemcpy2DAsync(d, (size_t)w * sizeof(T), src, (size_t)pitch * sizeof(T), (size_t)w * sizeof(T), h, cudaMemcpyHostToDevice, st));
+    *dev = d; *dpitch = w;
+    return VWB200_OK;
+  }
+  // an output `user` (may be NULL: scratch only): the caller's device raster itself -- when `dense` asks for it, only if its
+  // pitch is w -- or a dense HBM buffer that finish() copies to `user`, w elements per row so that the pitch padding is never
+  // written, unless *unless is set by then.  The buffer starts as a copy of `init` (an in-out raster passes itself), which
+  // lives where the call's inputs live.
+  template <class T> int out(T* user, int w, int h, ptrdiff_t pitch, int on_device, T** dev, ptrdiff_t* dpitch, const T* init = nullptr,
+                             ptrdiff_t ipitch = 0, bool dense = false, const int* unless = nullptr) {
+    if (on_device && user && (!init || init == user) && (!dense || pitch == w)) { *dev = user; *dpitch = pitch; return VWB200_OK; }
+    VWB_TRY(ar.alloc(dev, (size_t)w * h));
+    *dpitch = w;
+    const size_t row = (size_t)w * sizeof(T);
+    if (init)
+      VWB_CUDA(cudaMemcpy2DAsync(*dev, row, init, (size_t)ipitch * sizeof(T), row, h, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
+    if (user) backs.push_back(CopyBack{user, (size_t)pitch * sizeof(T), *dev, row, h, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, unless});
+    return VWB200_OK;
+  }
+  int finish() {
+    for (const CopyBack& b : backs)
+      if (!b.unless || !*b.unless) VWB_CUDA(cudaMemcpy2DAsync(b.dst, b.dpitch, b.src, b.row, b.row, b.h, b.kind, st));
+    VWB_CUDA(cudaStreamSynchronize(st));
+    return VWB200_OK;
+  }
+};
 
 // ---- disparity smoothing (Stereo/Algorithms.{h,cc}) ----------------------------------------------------------------
-// the two in-place filters: stage a host disparity through HBM, run the sweep, copy the result back, report a stall
+// the two in-place filters: run the sweep over the disparity (staged through HBM when on the host), report a stall
 template <class Run>
 static int smoothing_in_place(const char* what, float* disparity, int cols, int rows, ptrdiff_t pitch, int on_device, void* stream,
                               Run run) {
-  StreamGuard sg; VWB_TRY(sg.init(stream, on_device));
-  cudaStream_t st = sg.st;
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
   int stalled = 0;
-  {
-    Arena ar(st);
-    float* d = disparity; ptrdiff_t dp = pitch;
-    int* work;
-    VWB_TRY(ar.alloc(&work, (size_t)rows + 2));
-    if (!on_device) {
-      VWB_TRY(ar.alloc(&d, (size_t)cols * rows * 3));
-      dp = cols;
-      VWB_CUDA(cudaMemcpy2DAsync(d, (size_t)cols * 12, disparity, (size_t)pitch * 12, (size_t)cols * 12, rows, cudaMemcpyHostToDevice, st));
-    }
-    VWB_TRY(run(d, dp, work, &stalled, st));
-    if (!on_device)
-      VWB_CUDA(cudaMemcpy2DAsync(disparity, (size_t)pitch * 12, d, (size_t)cols * 12, (size_t)cols * 12, rows, cudaMemcpyDeviceToHost, st));
-  }
-  VWB_CUDA(cudaStreamSynchronize(st));
+  float* d; ptrdiff_t dp;
+  int* work;
+  VWB_TRY(c.ar.alloc(&work, (size_t)rows + 2));
+  VWB_TRY(c.out(disparity, cols * 3, rows, pitch * 3, on_device, &d, &dp, (const float*)disparity, pitch * 3));
+  VWB_TRY(run(c, d, dp / 3, work, &stalled));
+  VWB_TRY(c.finish());
   if (stalled) { set_error("%s: wavefront stalled (a row waited more than 10 s for the row above)", what); return VWB200_ELOGIC; }
   return VWB200_OK;
 }
@@ -1099,32 +1134,26 @@ int vwb200_calc_disparity(int cost_type, const float* left, int lw, int lh, ptrd
   if (!left || !right || !out) { set_error("calc_disparity: null pointer"); return VWB200_EARG; }
   if (lpitch < lw || rpitch < lw + sx - 1 || opitch < lw - kx + 1) { set_error("calc_disparity: a row pitch is smaller than its row"); return VWB200_EARG; }
   VWB_TRY(ensure_device());
-  StreamGuard sg; VWB_TRY(sg.init(stream, on_device));
-  cudaStream_t st = sg.st;
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
   const long long launches0 = g_launches.load();
   const int W = lw - kx + 1, H = lh - ky + 1;
   int path = 1;
   float kernel_ms = 0.0f;
   if (!on_device && (H > 1024 || getenv("VWB200_BAND_ROWS")) && !getenv("VWB200_NO_PIPELINE")) {
-    VWB_TRY(calc_disparity_host_pipelined(cost_type, left, lw, lh, lpitch, right, rpitch, sx, sy, kx, ky, out, opitch, st, &path, &kernel_ms));
+    VWB_TRY(calc_disparity_host_pipelined(cost_type, left, lw, lh, lpitch, right, rpitch, sx, sy, kx, ky, out, opitch, c.st, &path, &kernel_ms));
   } else {
     EventGuard evs;
     KEvents kev;
     VWB_TRY(evs.make(&kev.e0)); VWB_TRY(evs.make(&kev.e1));
-    {
-      Arena ar(st);
-      const float *dl, *dr; ptrdiff_t dlp, drp;
-      VWB_TRY(stage_in(left, lw, lh, lpitch, on_device, ar, st, &dl, &dlp));
-      VWB_TRY(stage_in(right, lw + sx - 1, lh + sy - 1, rpitch, on_device, ar, st, &dr, &drp));
-      vwb200_dispi* dout = out; ptrdiff_t dop = opitch;
-      if (!on_device) { VWB_TRY(ar.alloc(&dout, (size_t)W * H)); dop = W; }
-      const ImgF Li{dl, lw, lh, dlp}, Ri{dr, lw + sx - 1, lh + sy - 1, drp};
-      VWB_TRY(calc_disparity_device(cost_type, Li, Ri, W, H, sx, sy, kx, ky, dout, dop, ar, st, &kev, &path));
-      if (!on_device)
-        VWB_CUDA(cudaMemcpy2DAsync(out, (size_t)opitch * sizeof(vwb200_dispi), dout, (size_t)W * sizeof(vwb200_dispi),
-                                   (size_t)W * sizeof(vwb200_dispi), H, cudaMemcpyDeviceToHost, st));
-    }
-    VWB_CUDA(cudaStreamSynchronize(st));
+    const float *dl, *dr; ptrdiff_t dlp, drp;
+    VWB_TRY(c.in(left, lw, lh, lpitch, on_device, &dl, &dlp));
+    VWB_TRY(c.in(right, lw + sx - 1, lh + sy - 1, rpitch, on_device, &dr, &drp));
+    vwb200_dispi* dout; ptrdiff_t dop;
+    VWB_TRY(c.out(out, W, H, opitch, on_device, &dout, &dop));
+    const ImgF Li{dl, lw, lh, dlp}, Ri{dr, lw + sx - 1, lh + sy - 1, drp};
+    VWB_TRY(calc_disparity_device(cost_type, Li, Ri, W, H, sx, sy, kx, ky, dout, dop, c.ar, c.st, &kev, &path));
+    VWB_TRY(c.finish());
     if (cudaEventElapsedTime(&kernel_ms, kev.e0, kev.e1) != cudaSuccess) { kernel_ms = 0.0f; cudaGetLastError(); }
   }
   t_k1_stats.path = path;
@@ -1136,38 +1165,25 @@ int vwb200_calc_disparity(int cost_type, const float* left, int lw, int lh, ptrd
 int vwb200_pyramid_down(const float* in, int w, int h, ptrdiff_t pitch, float* out, ptrdiff_t opitch, int on_device, void* stream) {
   if (!in || !out || w <= 0 || h <= 0) { set_error("pyramid_down: bad arguments"); return VWB200_EARG; }
   VWB_TRY(ensure_device());
-  StreamGuard sg; VWB_TRY(sg.init(stream, on_device));
-  cudaStream_t st = sg.st;
-  {
-    Arena ar(st);
-    const int ow = 1 + (w - 1) / 2, oh = 1 + (h - 1) / 2;
-    const float* din; ptrdiff_t dp;
-    VWB_TRY(stage_in(in, w, h, pitch, on_device, ar, st, &din, &dp));
-    float* dout = out; ptrdiff_t dop = opitch;
-    if (!on_device) { VWB_TRY(ar.alloc(&dout, (size_t)ow * oh)); dop = ow; }
-    VWB_TRY(pyramid_down_launch(ImgF{din, w, h, dp}, dout, dop, st));
-    if (!on_device)
-      VWB_CUDA(cudaMemcpy2DAsync(out, (size_t)opitch * sizeof(float), dout, (size_t)ow * sizeof(float), (size_t)ow * sizeof(float), oh, cudaMemcpyDeviceToHost, st));
-  }
-  VWB_CUDA(cudaStreamSynchronize(st));
-  return VWB200_OK;
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
+  const float* din; ptrdiff_t dp;
+  VWB_TRY(c.in(in, w, h, pitch, on_device, &din, &dp));
+  float* dout; ptrdiff_t dop;
+  VWB_TRY(c.out(out, 1 + (w - 1) / 2, 1 + (h - 1) / 2, opitch, on_device, &dout, &dop));
+  VWB_TRY(pyramid_down_launch(ImgF{din, w, h, dp}, dout, dop, c.st));
+  return c.finish();
 }
 
 int vwb200_prefilter(const float* in, int w, int h, ptrdiff_t pitch, int mode, float width, float* out, ptrdiff_t opitch, int on_device, void* stream) {
   if (!in || !out || w <= 0 || h <= 0) { set_error("prefilter: bad arguments"); return VWB200_EARG; }
   VWB_TRY(ensure_device());
-  StreamGuard sg; VWB_TRY(sg.init(stream, on_device));
-  cudaStream_t st = sg.st;
-  {
-    Arena ar(st);
-    float* buf;
-    VWB_TRY(ar.alloc(&buf, (size_t)w * h));
-    VWB_CUDA(cudaMemcpy2DAsync(buf, (size_t)w * 4, in, (size_t)pitch * 4, (size_t)w * 4, h, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
-    VWB_TRY(prefilter_inplace(buf, w, h, mode, width, ar, st));
-    VWB_CUDA(cudaMemcpy2DAsync(out, (size_t)opitch * 4, buf, (size_t)w * 4, (size_t)w * 4, h, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
-    VWB_CUDA(cudaStreamSynchronize(st));
-  }
-  return VWB200_OK;
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
+  float* buf; ptrdiff_t bp;
+  VWB_TRY(c.out(out, w, h, opitch, on_device, &buf, &bp, in, pitch, /*dense=*/true));      // filtered in place: a dense copy of `in`
+  VWB_TRY(prefilter_inplace(buf, w, h, mode, width, c.ar, c.st));
+  return c.finish();
 }
 
 // calc_disparity_sgm behind the C ABI: stage the inputs, run vwb200::sgm_run, copy the results back
@@ -1190,69 +1206,37 @@ static int sgm_abi_run(const vwb200_sgm_params* sp, const float* left, int lw, i
   const int W = *out_w, H = *out_h;
   if ((out && opitch < W) || (out_sub && sub_pitch < W)) { set_error("sgm_calc_disparity: output pitch smaller than the output width"); return VWB200_EARG; }
   VWB_TRY(ensure_device());
-  StreamGuard sg; VWB_TRY(sg.init(stream, on_device));
-  cudaStream_t st = sg.st;
-  {
-    Arena ar(st);
-    SgmArgs a;
-    const float *dl, *dr; ptrdiff_t dlp, drp;
-    VWB_TRY(stage_in(left, lw, lh, lpitch, on_device, ar, st, &dl, &dlp));
-    VWB_TRY(stage_in(right, rw, rh, rpitch, on_device, ar, st, &dr, &drp));
-    a.left = ImgF{dl, lw, lh, dlp}; a.right = ImgF{dr, rw, rh, drp};
-    a.sx = search_x; a.sy = search_y; a.k = kernel_size;
-    a.ternary = sp->cost_type == VWB200_TERNARY_CENSUS_TRANSFORM; a.ternary_threshold = sp->ternary_threshold;
-    a.p1 = sp->p1; a.p2 = sp->p2; a.use_mgm = sp->use_mgm; a.subpixel_mode = out_sub ? sp->subpixel_mode : 0;
-    a.buf_x = sp->search_buffer_x; a.buf_y = sp->search_buffer_y; a.conserve_level = sp->conserve_level;
-    a.memory_limit_mb = sp->memory_limit_mb > 0 ? sp->memory_limit_mb : 6000.0;
-    a.assumed_threads = sp->assumed_threads > 0 ? sp->assumed_threads : 4;
-    if (W > 0 && H > 0) {
-      if (lmask) {
-        const uint8_t* d; ptrdiff_t dp;
-        VWB_TRY(stage_in(lmask, W, H, lmpitch, on_device, ar, st, &d, &dp));
-        a.lmask = ImgB{d, W, H, dp};
-      }
-      if (rmask) {
-        const uint8_t* d; ptrdiff_t dp;
-        VWB_TRY(stage_in(rmask, rmw, rmh, rmpitch, on_device, ar, st, &d, &dp));
-        a.rmask = ImgB{d, rmw, rmh, dp};
-      }
-      if (prev) {
-        if (pw <= 0 || ph <= 0) { set_error("sgm: empty previous disparity"); return VWB200_EARG; }
-        const vwb200_dispi* d; ptrdiff_t dp;
-        VWB_TRY(stage_in(prev, pw, ph, ppitch, on_device, ar, st, &d, &dp));
-        a.prev = d; a.pw = pw; a.ph = ph; a.ppitch = dp;
-      }
-      if (bounds) {
-        const int32_t* d; ptrdiff_t dp;
-        VWB_TRY(stage_in(bounds, W * 4, H, (ptrdiff_t)W * 4, on_device, ar, st, &d, &dp));
-        a.bounds_in = d;
-      }
-      vwb200_dispi* dout = out; ptrdiff_t dop = opitch;
-      if (!on_device || !out) { VWB_TRY(ar.alloc(&dout, (size_t)W * H)); dop = W; }
-      float* dsub = out_sub; ptrdiff_t dsp = sub_pitch * 3;
-      if (out_sub && !on_device) { VWB_TRY(ar.alloc(&dsub, (size_t)W * H * 3)); dsp = (ptrdiff_t)W * 3; }
-      int32_t* dbo = bounds_out;
-      if (bounds_out && !on_device) VWB_TRY(ar.alloc(&dbo, (size_t)W * H * 4));
-      a.out = dout; a.opitch = dop; a.out_sub = out_sub ? dsub : nullptr; a.sub_pitch = dsp; a.bounds_out = dbo;
-      VWB_TRY(sgm_run(a, ar, st));
-      if (!on_device && out)
-        VWB_CUDA(cudaMemcpy2DAsync(out, (size_t)opitch * sizeof(vwb200_dispi), dout, (size_t)W * sizeof(vwb200_dispi),
-                                   (size_t)W * sizeof(vwb200_dispi), H, cudaMemcpyDeviceToHost, st));
-      if (!on_device && out_sub)
-        VWB_CUDA(cudaMemcpy2DAsync(out_sub, (size_t)sub_pitch * 12, dsub, (size_t)W * 12, (size_t)W * 12, H, cudaMemcpyDeviceToHost, st));
-      if (!on_device && bounds_out)
-        VWB_CUDA(cudaMemcpyAsync(bounds_out, dbo, (size_t)W * H * 16, cudaMemcpyDeviceToHost, st));
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
+  SgmArgs a = sgm_args(*sp);
+  if (!out_sub) a.subpixel_mode = 0;
+  const float *dl, *dr; ptrdiff_t dlp, drp;
+  VWB_TRY(c.in(left, lw, lh, lpitch, on_device, &dl, &dlp));
+  VWB_TRY(c.in(right, rw, rh, rpitch, on_device, &dr, &drp));
+  a.left = ImgF{dl, lw, lh, dlp}; a.right = ImgF{dr, rw, rh, drp};
+  if (W > 0 && H > 0) {
+    ptrdiff_t dp;
+    if (lmask) { VWB_TRY(c.in(lmask, W, H, lmpitch, on_device, &a.lmask.p, &dp)); a.lmask = ImgB{a.lmask.p, W, H, dp}; }
+    if (rmask) { VWB_TRY(c.in(rmask, rmw, rmh, rmpitch, on_device, &a.rmask.p, &dp)); a.rmask = ImgB{a.rmask.p, rmw, rmh, dp}; }
+    if (prev) {
+      if (pw <= 0 || ph <= 0) { set_error("sgm: empty previous disparity"); return VWB200_EARG; }
+      VWB_TRY(c.in(prev, pw, ph, ppitch, on_device, &a.prev, &a.ppitch));
+      a.pw = pw; a.ph = ph;
     }
-    VWB_CUDA(cudaStreamSynchronize(st));
+    if (bounds) VWB_TRY(c.in(bounds, W * 4, H, (ptrdiff_t)W * 4, on_device, &a.bounds_in, &dp));
+    VWB_TRY(c.out(out, W, H, opitch, on_device, &a.out, &a.opitch));
+    if (out_sub) VWB_TRY(c.out(out_sub, W * 3, H, sub_pitch * 3, on_device, &a.out_sub, &a.sub_pitch));
+    if (bounds_out) VWB_TRY(c.out(bounds_out, W * 4, H, (ptrdiff_t)W * 4, on_device, &a.bounds_out, &dp));
+    VWB_TRY(sgm_run(a, c.ar, c.st));
   }
-  return VWB200_OK;
+  return c.finish();
 }
 
 static vwb200_sgm_params sgm_default_params(int search_x, int search_y, int kernel_size, int p1, int p2, int subpixel_mode) {
   vwb200_sgm_params sp{};
   sp.search_x = search_x; sp.search_y = search_y; sp.kernel_size = kernel_size; sp.cost_type = VWB200_CENSUS_TRANSFORM; sp.ternary_threshold = 5;
   sp.p1 = p1; sp.p2 = p2; sp.use_mgm = 0; sp.subpixel_mode = subpixel_mode; sp.search_buffer_x = 2; sp.search_buffer_y = 2; sp.conserve_level = -1;
-  sp.memory_limit_mb = 1e12; sp.assumed_threads = 4;
+  sp.memory_limit_mb = 1e12; sp.assumed_threads = kSgmThreads;
   return sp;
 }
 int vwb200_sgm_calc_disparity(const float* left, int lw, int lh, ptrdiff_t lpitch, const float* right, int rw, int rh, ptrdiff_t rpitch,
@@ -1285,24 +1269,17 @@ int vwb200_sgm_disp_bounds(const vwb200_sgm_params* sp, const vwb200_dispi* prev
                            int ow, int oh, int32_t* bounds, int on_device, void* stream) {
   if (!sp || !bounds || ow <= 0 || oh <= 0 || sp->search_x < 0 || sp->search_y < 0) { set_error("sgm_disp_bounds: bad arguments"); return VWB200_EARG; }
   VWB_TRY(ensure_device());
-  StreamGuard sg; VWB_TRY(sg.init(stream, on_device));
-  cudaStream_t st = sg.st;
-  {
-    Arena ar(st);
-    SgmArgs a;
-    a.sx = sp->search_x; a.sy = sp->search_y; a.buf_x = sp->search_buffer_x; a.buf_y = sp->search_buffer_y; a.conserve_level = sp->conserve_level;
-    a.use_mgm = sp->use_mgm; a.memory_limit_mb = sp->memory_limit_mb > 0 ? sp->memory_limit_mb : 6000.0;
-    a.assumed_threads = sp->assumed_threads > 0 ? sp->assumed_threads : 4;
-    if (lmask) { const uint8_t* d; ptrdiff_t dp; VWB_TRY(stage_in(lmask, ow, oh, lmpitch, on_device, ar, st, &d, &dp)); a.lmask = ImgB{d, ow, oh, dp}; }
-    if (rmask) { const uint8_t* d; ptrdiff_t dp; VWB_TRY(stage_in(rmask, rmw, rmh, rmpitch, on_device, ar, st, &d, &dp)); a.rmask = ImgB{d, rmw, rmh, dp}; }
-    if (prev) { const vwb200_dispi* d; ptrdiff_t dp; VWB_TRY(stage_in(prev, pw, ph, ppitch, on_device, ar, st, &d, &dp)); a.prev = d; a.pw = pw; a.ph = ph; a.ppitch = dp; }
-    int32_t* db = bounds;
-    if (!on_device) VWB_TRY(ar.alloc(&db, (size_t)ow * oh * 4));
-    VWB_TRY(sgm_bounds_run(a, ow, oh, db, ar, st));
-    if (!on_device) VWB_CUDA(cudaMemcpyAsync(bounds, db, (size_t)ow * oh * 16, cudaMemcpyDeviceToHost, st));
-    VWB_CUDA(cudaStreamSynchronize(st));
-  }
-  return VWB200_OK;
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
+  SgmArgs a = sgm_args(*sp);
+  ptrdiff_t dp;
+  if (lmask) { VWB_TRY(c.in(lmask, ow, oh, lmpitch, on_device, &a.lmask.p, &dp)); a.lmask = ImgB{a.lmask.p, ow, oh, dp}; }
+  if (rmask) { VWB_TRY(c.in(rmask, rmw, rmh, rmpitch, on_device, &a.rmask.p, &dp)); a.rmask = ImgB{a.rmask.p, rmw, rmh, dp}; }
+  if (prev) { VWB_TRY(c.in(prev, pw, ph, ppitch, on_device, &a.prev, &a.ppitch)); a.pw = pw; a.ph = ph; }
+  int32_t* db;
+  VWB_TRY(c.out(bounds, ow * 4, oh, (ptrdiff_t)ow * 4, on_device, &db, &dp));
+  VWB_TRY(sgm_bounds_run(a, ow, oh, db, c.ar, c.st));
+  return c.finish();
 }
 
 int vwb200_parabola_subpixel(const float* disparity, int cols, int rows, const float* left, ptrdiff_t lpitch,
@@ -1313,38 +1290,32 @@ int vwb200_parabola_subpixel(const float* disparity, int cols, int rows, const f
   if (x1 <= x0 || y1 <= y0 || x0 < 0 || y0 < 0 || x1 > cols || y1 > rows) { set_error("parabola_subpixel: bbox outside the disparity image"); return VWB200_EARG; }
   if (kx % 2 != 1 || ky % 2 != 1 || kx < 1 || ky < 1) { set_error("parabola_subpixel: kernel size must be odd"); return VWB200_EARG; }
   VWB_TRY(ensure_device());
-  StreamGuard sg; VWB_TRY(sg.init(stream, on_device));
-  cudaStream_t st = sg.st;
-  {
-    Arena ar(st);
-    const int bw = x1 - x0, bh = y1 - y0;
-    const float *dd, *dl, *dr; ptrdiff_t p0, p1, p2;
-    VWB_TRY(stage_in(disparity, cols * 3, rows, (ptrdiff_t)cols * 3, on_device, ar, st, &dd, &p0));
-    VWB_TRY(stage_in(left, cols, rows, lpitch, on_device, ar, st, &dl, &p1));
-    VWB_TRY(stage_in(right, rcols, rrows, rpitch, on_device, ar, st, &dr, &p2));
-    int* d_r; int hr[5];
-    VWB_TRY(ar.alloc(&d_r, 5));
-    VWB_TRY(disp_range_launch(dd, cols, x0, y0, bw, bh, d_r, st));
-    VWB_CUDA(cudaMemcpyAsync(hr, d_r, sizeof(hr), cudaMemcpyDeviceToHost, st));
-    VWB_CUDA(cudaStreamSynchronize(st));
-    if (!hr[4]) { hr[0] = hr[1] = hr[2] = hr[3] = 0; }
-    // entire_search_range: max += 1, expand(1)  (ParabolaSubpixelView.cc:296-299)
-    const Box sr{hr[0] - 1, hr[1] - 1, hr[2] + 2, hr[3] + 2};
-    const int hkx = kx / 2, hky = ky / 2;
-    const Box lreg{x0 - hkx, y0 - hky, x1 + hkx, y1 + hky};
-    const Box rreg{lreg.x0 + sr.x0, lreg.y0 + sr.y0, lreg.x1 + sr.x0 + (sr.x1 - sr.x0), lreg.y1 + sr.y0 + (sr.y1 - sr.y0)};
-    float *Lf, *Rf;
-    VWB_TRY(filtered_region(ImgF{dl, cols, rows, p1}, prefilter_mode, prefilter_width, lreg, &Lf, ar, st));
-    VWB_TRY(filtered_region(ImgF{dr, rcols, rrows, p2}, prefilter_mode, prefilter_width, rreg, &Rf, ar, st));
-    float* dout = dest;
-    if (!on_device || dest_pitch != bw) VWB_TRY(ar.alloc(&dout, (size_t)bw * bh * 3));
-    VWB_TRY(parabola_launch(dd, cols, x0, y0, bw, bh, Lf, lreg.x1 - lreg.x0, Rf, rreg.x1 - rreg.x0, sr.x0, sr.y0, kx, ky, dout, st));
-    if (dout != dest)
-      VWB_CUDA(cudaMemcpy2DAsync(dest, (size_t)dest_pitch * 12, dout, (size_t)bw * 12, (size_t)bw * 12, bh,
-                                 on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
-    VWB_CUDA(cudaStreamSynchronize(st));
-  }
-  return VWB200_OK;
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
+  cudaStream_t st = c.st;
+  const int bw = x1 - x0, bh = y1 - y0;
+  const float *dd, *dl, *dr; ptrdiff_t p0, p1, p2;
+  VWB_TRY(c.in(disparity, cols * 3, rows, (ptrdiff_t)cols * 3, on_device, &dd, &p0));
+  VWB_TRY(c.in(left, cols, rows, lpitch, on_device, &dl, &p1));
+  VWB_TRY(c.in(right, rcols, rrows, rpitch, on_device, &dr, &p2));
+  int* d_r; int hr[5];
+  VWB_TRY(c.ar.alloc(&d_r, 5));
+  VWB_TRY(disp_range_launch(dd, cols, x0, y0, bw, bh, d_r, st));
+  VWB_CUDA(cudaMemcpyAsync(hr, d_r, sizeof(hr), cudaMemcpyDeviceToHost, st));
+  VWB_CUDA(cudaStreamSynchronize(st));
+  if (!hr[4]) { hr[0] = hr[1] = hr[2] = hr[3] = 0; }
+  // entire_search_range: max += 1, expand(1)  (ParabolaSubpixelView.cc:296-299)
+  const Box sr{hr[0] - 1, hr[1] - 1, hr[2] + 2, hr[3] + 2};
+  const int hkx = kx / 2, hky = ky / 2;
+  const Box lreg{x0 - hkx, y0 - hky, x1 + hkx, y1 + hky};
+  const Box rreg{lreg.x0 + sr.x0, lreg.y0 + sr.y0, lreg.x1 + sr.x0 + (sr.x1 - sr.x0), lreg.y1 + sr.y0 + (sr.y1 - sr.y0)};
+  float *Lf, *Rf;
+  VWB_TRY(filtered_region(ImgF{dl, cols, rows, p1}, prefilter_mode, prefilter_width, lreg, &Lf, c.ar, st));
+  VWB_TRY(filtered_region(ImgF{dr, rcols, rrows, p2}, prefilter_mode, prefilter_width, rreg, &Rf, c.ar, st));
+  float* dout; ptrdiff_t dop;
+  VWB_TRY(c.out(dest, bw * 3, bh, dest_pitch * 3, on_device, &dout, &dop, (const float*)nullptr, 0, /*dense=*/true));
+  VWB_TRY(parabola_launch(dd, cols, x0, y0, bw, bh, Lf, lreg.x1 - lreg.x0, Rf, rreg.x1 - rreg.x0, sr.x0, sr.y0, kx, ky, dout, st));
+  return c.finish();
 }
 
 int vwb200_disparity_median_filter(float* disparity, int cols, int rows, ptrdiff_t pitch, int kernel_size, int on_device, void* stream) {
@@ -1355,8 +1326,8 @@ int vwb200_disparity_median_filter(float* disparity, int cols, int rows, ptrdiff
   const int half = (kernel_size - 1) / 2;
   if (kernel_size < 3 || cols <= 2 * half || rows <= 2 * half) return VWB200_OK;     // Algorithms.cc:34-35: nothing to filter
   return smoothing_in_place(what, disparity, cols, rows, pitch, on_device, stream,
-                            [&](float* d, ptrdiff_t dp, int* work, int* err, cudaStream_t st) {
-                              return median_sweep_launch(d, cols, rows, dp, kernel_size, work, err, st);
+                            [&](AbiCall& c, float* d, ptrdiff_t dp, int* work, int* err) {
+                              return median_sweep_launch(d, cols, rows, dp, kernel_size, work, err, c.st);
                             });
 }
 
@@ -1368,20 +1339,14 @@ int vwb200_texture_measure(const float* image, int cols, int rows, ptrdiff_t pit
   if (kernel_size > kSmoothMaxKernel) { set_error("texture_measure: kernel_size %d is above the supported %d", kernel_size, kSmoothMaxKernel); return VWB200_ENOIMPL; }
   VWB_TRY(ensure_device());
   if (!cols || !rows) return VWB200_OK;
-  StreamGuard sg; VWB_TRY(sg.init(stream, on_device));
-  cudaStream_t st = sg.st;
-  {
-    Arena ar(st);
-    const float* din; ptrdiff_t dp;
-    VWB_TRY(stage_in(image, cols, rows, pitch, on_device, ar, st, &din, &dp));
-    float* dout = out; ptrdiff_t dop = opitch;
-    if (!on_device) { VWB_TRY(ar.alloc(&dout, (size_t)cols * rows)); dop = cols; }
-    VWB_TRY(texture_measure_launch(ImgF{din, cols, rows, dp}, kernel_size, gradient_weight, stddev_weight, dout, dop, st));
-    if (!on_device)
-      VWB_CUDA(cudaMemcpy2DAsync(out, (size_t)opitch * 4, dout, (size_t)cols * 4, (size_t)cols * 4, rows, cudaMemcpyDeviceToHost, st));
-  }
-  VWB_CUDA(cudaStreamSynchronize(st));
-  return VWB200_OK;
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
+  const float* din; ptrdiff_t dp;
+  VWB_TRY(c.in(image, cols, rows, pitch, on_device, &din, &dp));
+  float* dout; ptrdiff_t dop;
+  VWB_TRY(c.out(out, cols, rows, opitch, on_device, &dout, &dop));
+  VWB_TRY(texture_measure_launch(ImgF{din, cols, rows, dp}, kernel_size, gradient_weight, stddev_weight, dout, dop, c.st));
+  return c.finish();
 }
 
 int vwb200_texture_preserving_disparity_filter(float* disparity, int cols, int rows, ptrdiff_t pitch, const float* texture,
@@ -1393,86 +1358,58 @@ int vwb200_texture_preserving_disparity_filter(float* disparity, int cols, int r
   VWB_TRY(ensure_device());
   if (max_kernel_size < 3 || texture_max <= 0 || !cols || !rows) return VWB200_OK;   // Algorithms.h:228-229
   return smoothing_in_place(what, disparity, cols, rows, pitch, on_device, stream,
-                            [&](float* d, ptrdiff_t dp, int* work, int* err, cudaStream_t st) -> int {
-                              Arena ar(st);
+                            [&](AbiCall& c, float* d, ptrdiff_t dp, int* work, int* err) -> int {
                               const float* t; ptrdiff_t tp;
-                              VWB_TRY(stage_in(texture, cols, rows, tpitch, on_device, ar, st, &t, &tp));
-                              return texture_filter_sweep_launch(d, cols, rows, dp, t, tp, texture_max, max_kernel_size, work, err, st);
+                              VWB_TRY(c.in(texture, cols, rows, tpitch, on_device, &t, &tp));
+                              return texture_filter_sweep_launch(d, cols, rows, dp, t, tp, texture_max, max_kernel_size, work, err, c.st);
                             });
 }
 
 int vwb200_subsample_mask_by_two(const uint8_t* in, int w, int h, ptrdiff_t pitch, uint8_t* out, ptrdiff_t opitch, int on_device, void* stream) {
   if (!in || !out || w <= 0 || h <= 0) { set_error("subsample_mask_by_two: bad arguments"); return VWB200_EARG; }
   VWB_TRY(ensure_device());
-  StreamGuard sg; VWB_TRY(sg.init(stream, on_device));
-  cudaStream_t st = sg.st;
-  {
-    Arena ar(st);
-    const int ow = 1 + (w - 1) / 2, oh = 1 + (h - 1) / 2;
-    const uint8_t* din; ptrdiff_t dp;
-    VWB_TRY(stage_in(in, w, h, pitch, on_device, ar, st, &din, &dp));
-    uint8_t* dout = out; ptrdiff_t dop = opitch;
-    if (!on_device) { VWB_TRY(ar.alloc(&dout, (size_t)ow * oh)); dop = ow; }
-    VWB_TRY(subsample_mask_launch(ImgB{din, w, h, dp}, dout, dop, st));
-    if (!on_device)
-      VWB_CUDA(cudaMemcpy2DAsync(out, (size_t)opitch, dout, (size_t)ow, (size_t)ow, oh, cudaMemcpyDeviceToHost, st));
-  }
-  VWB_CUDA(cudaStreamSynchronize(st));
-  return VWB200_OK;
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
+  const uint8_t* din; ptrdiff_t dp;
+  VWB_TRY(c.in(in, w, h, pitch, on_device, &din, &dp));
+  uint8_t* dout; ptrdiff_t dop;
+  VWB_TRY(c.out(out, 1 + (w - 1) / 2, 1 + (h - 1) / 2, opitch, on_device, &dout, &dop));
+  VWB_TRY(subsample_mask_launch(ImgB{din, w, h, dp}, dout, dop, c.st));
+  return c.finish();
 }
 
 int vwb200_cross_corr_consistency_check(vwb200_dispi* l2r, int lw, int lh, ptrdiff_t lpitch, const vwb200_dispi* r2l, int rw, int rh,
                                         ptrdiff_t rpitch, float threshold, int on_device, void* stream) {
   if (!l2r || !r2l) { set_error("cross_corr_consistency_check: null pointer"); return VWB200_EARG; }
   VWB_TRY(ensure_device());
-  StreamGuard sg; VWB_TRY(sg.init(stream, on_device));
-  cudaStream_t st = sg.st;
-  {
-    Arena ar(st);
-    vwb200_dispi* dl = l2r; const vwb200_dispi* dr = r2l; ptrdiff_t dlp = lpitch, drp = rpitch;
-    if (!on_device) {
-      VWB_TRY(ar.alloc(&dl, (size_t)lw * lh));
-      VWB_CUDA(cudaMemcpy2DAsync(dl, (size_t)lw * 12, l2r, (size_t)lpitch * 12, (size_t)lw * 12, lh, cudaMemcpyHostToDevice, st));
-      dlp = lw;
-      VWB_TRY(stage_in(r2l, rw, rh, rpitch, 0, ar, st, &dr, &drp));
-    }
-    VWB_TRY(consistency_launch(dl, lw, lh, dlp, dr, rw, rh, drp, threshold, st));
-    if (!on_device)
-      VWB_CUDA(cudaMemcpy2DAsync(l2r, (size_t)lpitch * 12, dl, (size_t)lw * 12, (size_t)lw * 12, lh, cudaMemcpyDeviceToHost, st));
-  }
-  VWB_CUDA(cudaStreamSynchronize(st));
-  return VWB200_OK;
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
+  vwb200_dispi* dl; const vwb200_dispi* dr; ptrdiff_t dlp, drp;
+  VWB_TRY(c.out(l2r, lw, lh, lpitch, on_device, &dl, &dlp, (const vwb200_dispi*)l2r, lpitch));
+  VWB_TRY(c.in(r2l, rw, rh, rpitch, on_device, &dr, &drp));
+  VWB_TRY(consistency_launch(dl, lw, lh, dlp, dr, rw, rh, drp, threshold, c.st));
+  return c.finish();
 }
 
+// the outlier filters and the mask on dense w x h rasters
 static int filter_common(int which, const vwb200_dispi* in, int w, int h, int hx, int hy, double pt, double rt,
                          const uint8_t* lm, const uint8_t* rm, int rmw, int rmh, vwb200_dispi* out, int on_device, void* stream) {
   if (!in || !out || w <= 0 || h <= 0) { set_error("disparity filter: bad arguments"); return VWB200_EARG; }
   VWB_TRY(ensure_device());
-  StreamGuard sg; VWB_TRY(sg.init(stream, on_device));
-  cudaStream_t st = sg.st;
-  {
-    Arena ar(st);
-    const vwb200_dispi* din; ptrdiff_t dp;
-    VWB_TRY(stage_in(in, w, h, (ptrdiff_t)w, on_device, ar, st, &din, &dp));
-    vwb200_dispi* dout = out;
-    if (!on_device) VWB_TRY(ar.alloc(&dout, (size_t)w * h));
-    if (which == 0) {
-      VWB_TRY(rm_outliers_launch(din, w, h, hx, hy, pt, rt, 0, 0, w, h, dout, st));
-    } else if (which == 1) {
-      vwb200_dispi* t1;
-      VWB_TRY(ar.alloc(&t1, (size_t)(w + 2) * (h + 2)));
-      VWB_TRY(rm_outliers_launch(din, w, h, hx, hy, pt, rt, -1, -1, w + 2, h + 2, t1, st));
-      VWB_TRY(cleanup_pass2_launch(t1, w, h, dout, st));
-    } else {
-      const uint8_t *dlm, *drm; ptrdiff_t p1, p2;
-      VWB_TRY(stage_in(lm, w, h, (ptrdiff_t)w, on_device, ar, st, &dlm, &p1));
-      VWB_TRY(stage_in(rm, rmw, rmh, (ptrdiff_t)rmw, on_device, ar, st, &drm, &p2));
-      VWB_TRY(disparity_mask_launch(din, w, h, ImgB{dlm, w, h, p1}, ImgB{drm, rmw, rmh, p2}, dout, st));
-    }
-    if (!on_device) VWB_CUDA(cudaMemcpyAsync(out, dout, (size_t)w * h * sizeof(vwb200_dispi), cudaMemcpyDeviceToHost, st));
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
+  const vwb200_dispi* din; vwb200_dispi* dout; ptrdiff_t dp;
+  VWB_TRY(c.in(in, w, h, (ptrdiff_t)w, on_device, &din, &dp));
+  VWB_TRY(c.out(out, w, h, (ptrdiff_t)w, on_device, &dout, &dp));
+  if (which < 2) {
+    VWB_TRY(outlier_filter_chain(din, w, h, hx, hy, pt, rt, which == 1, ImgB{}, ImgB{}, dout, c.ar, c.st));
+  } else {
+    const uint8_t *dlm, *drm; ptrdiff_t p1, p2;
+    VWB_TRY(c.in(lm, w, h, (ptrdiff_t)w, on_device, &dlm, &p1));
+    VWB_TRY(c.in(rm, rmw, rmh, (ptrdiff_t)rmw, on_device, &drm, &p2));
+    VWB_TRY(disparity_mask_launch(din, w, h, ImgB{dlm, w, h, p1}, ImgB{drm, rmw, rmh, p2}, dout, c.st));
   }
-  VWB_CUDA(cudaStreamSynchronize(st));
-  return VWB200_OK;
+  return c.finish();
 }
 int vwb200_rm_outliers_using_thresh(const vwb200_dispi* in, int w, int h, int hx, int hy, double pt, double rt, vwb200_dispi* out, int on_device, void* stream) {
   return filter_common(0, in, w, h, hx, hy, pt, rt, nullptr, nullptr, 0, 0, out, on_device, stream);
@@ -1558,48 +1495,37 @@ static int corr_rasterize_impl(vwb200_corr* h, int x0, int y0, int x1, int y1, f
   cudaGetDevice(&prev_dev);
   struct DevRestore { int d; ~DevRestore() { if (d >= 0) cudaSetDevice(d); } } restore{prev_dev != h->device ? prev_dev : -1};
   VWB_CUDA(cudaSetDevice(h->device));
-  StreamGuard sg; VWB_TRY(sg.init(stream, ((h->owned || h->streamed) ? dest_on_device : 1)));
-  cudaStream_t st = sg.st;
-  {
-    Arena ar(st);
-    const int bw = x1 - x0, bh = y1 - y0;
-    Box proc{x0, y0, x1, y1};
-    if (with_collar && h->p.collar_size > 0) proc = bexpand(proc, h->p.collar_size, h->p.collar_size);   // CorrelationView.h:128-131
-    const int pw = proc.x1 - proc.x0, ph = proc.y1 - proc.y0;
-    vwb200_corr::DiffTile df;
-    float* host_diff_window = nullptr;
-    if (h->diff) {                                                                                        // CorrelationView.cc:276-283
-      const int ulx = h->p.region_ul_x, uly = h->p.region_ul_y;
-      if (!(proc.x0 >= ulx && proc.y0 >= uly && proc.x1 <= ulx + h->diff_cols && proc.y1 <= uly + h->diff_rows)) {
-        set_error("The L-R to R-L difference image domain does not contain the current tile.");
-        return VWB200_EARG;
-      }
-      if (h->diff_on_device) { df.d = h->diff; df.pitch = h->diff_pitch; df.ox = proc.x0 - ulx; df.oy = proc.y0 - uly; }
-      else {                        // stage the tile's window (pixels the tile does not write keep their content)
-        host_diff_window = h->diff + ((ptrdiff_t)(proc.y0 - uly) * h->diff_pitch + (proc.x0 - ulx)) * 2;
-        VWB_TRY(ar.alloc(&df.d, (size_t)pw * ph * 2));
-        df.pitch = pw; df.ox = 0; df.oy = 0;
-        VWB_CUDA(cudaMemcpy2DAsync(df.d, (size_t)pw * 8, host_diff_window, (size_t)h->diff_pitch * 8, (size_t)pw * 8, ph, cudaMemcpyHostToDevice, st));
-      }
+  AbiCall c;
+  VWB_TRY(c.open(stream, (h->owned || h->streamed) ? dest_on_device : 1));
+  const int bw = x1 - x0, bh = y1 - y0;
+  Box proc{x0, y0, x1, y1};
+  if (with_collar && h->p.collar_size > 0) proc = bexpand(proc, h->p.collar_size, h->p.collar_size);   // CorrelationView.h:128-131
+  const int pw = proc.x1 - proc.x0, ph = proc.y1 - proc.y0;
+  vwb200_corr::DiffTile df;
+  vwb200_dispi* disp = nullptr; float* sub = nullptr; int all_invalid = 0;
+  if (h->diff) {                                                                                        // CorrelationView.cc:276-283
+    const int ulx = h->p.region_ul_x, uly = h->p.region_ul_y;
+    if (!(proc.x0 >= ulx && proc.y0 >= uly && proc.x1 <= ulx + h->diff_cols && proc.y1 <= uly + h->diff_rows)) {
+      set_error("The L-R to R-L difference image domain does not contain the current tile.");
+      return VWB200_EARG;
     }
-    vwb200_dispi* disp = nullptr; float* sub = nullptr; int all_invalid = 0;
-    VWB_TRY(h->prerasterize(proc, &disp, &sub, &all_invalid, df, ar, st));
-    float* dout = dest; ptrdiff_t dop = dest_pitch;
-    if (!dest_on_device) { VWB_TRY(ar.alloc(&dout, (size_t)bw * bh * 3)); dop = bw; }
-    if (all_invalid) {
-      VWB_CUDA(cudaMemset2DAsync(dout, (size_t)dop * 12, 0, (size_t)bw * 12, bh, st));
-    } else if (sgm) {
-      VWB_TRY(sgm_finalize_launch(sub, disp, pw, h->p.search_x0, h->p.search_y0, dout, dop, x0 - proc.x0, y0 - proc.y0, bw, bh, st));
-    } else {
-      VWB_TRY(finalize_launch(disp, pw, ph, h->p.search_x0, h->p.search_y0, dout, dop, x0 - proc.x0, y0 - proc.y0, bw, bh, st));
-    }
-    if (!dest_on_device)
-      VWB_CUDA(cudaMemcpy2DAsync(dest, (size_t)dest_pitch * 12, dout, (size_t)bw * 12, (size_t)bw * 12, bh, cudaMemcpyDeviceToHost, st));
-    if (host_diff_window && !all_invalid)
-      VWB_CUDA(cudaMemcpy2DAsync(host_diff_window, (size_t)h->diff_pitch * 8, df.d, (size_t)pw * 8, (size_t)pw * 8, ph, cudaMemcpyDeviceToHost, st));
-    VWB_CUDA(cudaStreamSynchronize(st));
+    // the tile's window; pixels the tile does not write keep their content, and an all-invalid tile leaves it alone
+    float* window = h->diff + ((ptrdiff_t)(proc.y0 - uly) * h->diff_pitch + (proc.x0 - ulx)) * 2;
+    VWB_TRY(c.out(window, pw * 2, ph, h->diff_pitch * 2, h->diff_on_device, &df.d, &df.pitch, (const float*)window, h->diff_pitch * 2, false,
+                  &all_invalid));
+    df.pitch /= 2;
   }
-  return VWB200_OK;
+  float* dout; ptrdiff_t dop;
+  VWB_TRY(c.out(dest, bw * 3, bh, dest_pitch * 3, dest_on_device, &dout, &dop));
+  VWB_TRY(h->prerasterize(proc, &disp, &sub, &all_invalid, df, c.ar, c.st));
+  if (all_invalid) {
+    VWB_CUDA(cudaMemset2DAsync(dout, (size_t)dop * 4, 0, (size_t)bw * 12, bh, c.st));
+  } else if (sgm) {
+    VWB_TRY(sgm_finalize_launch(sub, disp, pw, h->p.search_x0, h->p.search_y0, dout, dop / 3, x0 - proc.x0, y0 - proc.y0, bw, bh, c.st));
+  } else {
+    VWB_TRY(finalize_launch(disp, pw, ph, h->p.search_x0, h->p.search_y0, dout, dop / 3, x0 - proc.x0, y0 - proc.y0, bw, bh, c.st));
+  }
+  return c.finish();
 }
 int vwb200_corr_rasterize(vwb200_corr* h, int x0, int y0, int x1, int y1, float* dest, ptrdiff_t dest_pitch, int dest_on_device, void* stream) {
   return corr_rasterize_impl(h, x0, y0, x1, y1, dest, dest_pitch, dest_on_device, stream, true);
