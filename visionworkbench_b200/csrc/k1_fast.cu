@@ -7,14 +7,15 @@
 // dx-minor order => first disparity wins ties; all-equal => invalid), so it is bit-identical to the
 // reference while doing ~10 issue slots per (pixel, disparity) instead of ~70 bytes of DRAM traffic.
 //
-// Decomposition (persistent CTAs of 8 warps, one CTA per SM; work item = 236-column x th-row band, th chosen by
-// fast_geom within the shared-memory budget -- 84 rows at 128 x 128 / 21 x 21):
+// Decomposition (persistent CTAs of 12 warps at <= 168 registers, one CTA per SM = 3 warps per sub-partition; work
+// item = 236-column x th-row band, th chosen by fast_geom within the shared-memory budget -- 84 rows at 128 x 128 / 21 x 21):
 //   * values are pre-packed (pack kernels) as u16 (v-vmin)*8, one contiguous row per strip, so that a
 //     lane fetches its 8 left / 16 right columns with conflict-free 16-byte LDS.128 loads
 //   * the left tile (th+ky-1 rows) and a ring of right rows are staged in shared memory with TMA bulk
-//     copies (cp.async.bulk + mbarrier); one new right row is prefetched per dy while the CTA computes
-//   * warp w takes the dx octets w, w+8, ... and slides each over every row of the band, so the ky rows
-//     that seed its vertical sums are summed once per (dy, octet) and band
+//     copies (cp.async.bulk + mbarrier); the dy range runs in periods of sd (<= 3) dy rows with one barrier each,
+//     and the next period's sd right rows are prefetched while the CTA computes
+//   * a period's work units are its (dy, octet) pairs; warp w takes units w, w+12, ... and slides each over every
+//     row of the band, so the ky rows that seed its vertical sums are summed once per (dy, octet) and band
 //   * lane l owns padded columns 8l..8l+7 and 8 consecutive dx: V[8][8] vertical sliding sums live in
 //     registers (VABSDIFF accumulate: +new row, -old row)
 //   * the kx-wide horizontal sums are formed without shared memory: in-lane prefix sums + 9 warp
@@ -79,13 +80,32 @@ int image_stats_launch(ImgF img, float* d_result3, cudaStream_t st) {
 }
 
 // ---- band geometry ------------------------------------------------------------------------------------------------
+static constexpr int FK_WARPS = 12;                  // per CTA: 3 per SM sub-partition, at most 168 registers per thread
+static constexpr int FK_THREADS = FK_WARPS * 32;
+static constexpr int FK_SD_MAX = 3;                  // dy rows per synchronisation period (ring depth)
 static constexpr int FK_TH_MAX = 96;                 // tallest band considered
 static constexpr size_t FK_SMEM = 227 * 1024;
 static constexpr uint32_t FK_INIT_HI = 0x7fffffffu;  // high word of an empty key: above every (cost*8 | 7)
 
-// best plane [th][256] (u32) | left tile [th+ky-1][256] (u16) | right ring [th+ky][rw] (u16) | 2 mbarriers
+// best plane [th][256] (u32) | left tile [th+ky-1][256] (u16) | right ring [ring_slots][rw] (u16) | 2 mbarriers
 static size_t fast_smem_bytes(const FastGeom& g) {
   return (size_t)g.th * F_COLS * 4 + (size_t)g.ltile_rows * F_COLS * 2 + (size_t)g.ring_slots * g.rw * 2 + 64;
+}
+
+// A period of sd dy rows is ngroups * sd work units (one (dy, octet) pass each), dealt statically to the 12 warps:
+// take the depth whose units fill the warps best (48 units = 4 per warp at 16 octets), the deeper one on a tie (fewer
+// barriers).  The ring holds the period's ltile_rows + sd - 1 right rows while the next period's sd rows arrive.
+static FastGeom fast_make_geom(int W, int H, int sx, int sy, int kx, int ky, int th) {
+  FastGeom g = make_geom(W, H, sx, sy, kx, ky, th);
+  const int ngroups = (sx + F_B - 1) / F_B;
+  double best = -1.0;
+  for (int sd = 1; sd <= FK_SD_MAX && sd <= g.dy_per; ++sd) {
+    const int units = ngroups * sd;
+    const double eff = (double)units / (double)(((units + FK_WARPS - 1) / FK_WARPS) * FK_WARPS);
+    if (eff >= best - 1e-9) { best = eff; g.sd = sd; }
+  }
+  g.ring_slots = g.ltile_rows + 2 * g.sd - 1;
+  return g;
 }
 
 // Band height: a taller band spreads the seeding of each (dy, octet) -- ky rows of vertical sums plus a first row
@@ -93,10 +113,10 @@ static size_t fast_smem_bytes(const FastGeom& g) {
 // the height between F_TH and what the shared memory holds with the least estimated time: waves of work items x
 // row steps per item (make_geom picks the dy chunking J for each height).
 static FastGeom fast_geom(int W, int H, int sx, int sy, int kx, int ky) {
-  FastGeom best = make_geom(W, H, sx, sy, kx, ky, F_TH);
+  FastGeom best = fast_make_geom(W, H, sx, sy, kx, ky, F_TH);
   double tbest = -1.0;
   for (int th = F_TH; th <= FK_TH_MAX; ++th) {
-    const FastGeom g = make_geom(W, H, sx, sy, kx, ky, th);
+    const FastGeom g = fast_make_geom(W, H, sx, sy, kx, ky, th);
     if (fast_smem_bytes(g) > FK_SMEM) break;
     const long long waves = ((long long)g.NS * g.NB * g.J + kNumSMs - 1) / kNumSMs;
     const double t = (double)waves * g.dy_per * ((th < H ? th : H) + 0.15 * ky) * (1.0 + 0.004 * (g.J - 1));
@@ -119,7 +139,7 @@ int k1_fast_supported(int cost, int kx, int ky, int sx, int sy, float vmin, floa
   if (sx < F_B || sx > 512 || sy < 1) return VWB200_ENOIMPL;
   if ((long long)sx * sy > 65536) return VWB200_ENOIMPL;
   if ((long long)sx * sy < 64) return VWB200_ENOIMPL;      // tiny searches: the generic kernel is as good
-  if (fast_smem_bytes(make_geom(256, F_TH, sx, sy, kx, ky, F_TH)) > FK_SMEM) return VWB200_ENOIMPL;
+  if (fast_smem_bytes(fast_make_geom(256, F_TH, sx, sy, kx, ky, F_TH)) > FK_SMEM) return VWB200_ENOIMPL;
   return VWB200_OK;
 }
 
@@ -333,7 +353,7 @@ __device__ __forceinline__ void fast_pass_sq(const uint16_t* __restrict__ ltile,
 }
 
 template <int KX, bool SQ = false>
-__global__ void __launch_bounds__(F_THREADS, 1)
+__global__ void __launch_bounds__(FK_THREADS, 1)
 k1_fast_abs_kernel(const uint16_t* __restrict__ L16, const uint16_t* __restrict__ R16, FastGeom G,
                    vwb200_dispi* __restrict__ out, ptrdiff_t opitch, uint32_t* __restrict__ part_cost, uint16_t* __restrict__ part_idx,
                    unsigned long long* __restrict__ gkeys) {
@@ -344,7 +364,7 @@ k1_fast_abs_kernel(const uint16_t* __restrict__ L16, const uint16_t* __restrict_
   uint16_t* rring = ltile + (size_t)G.ltile_rows * F_COLS;
   uint64_t* bars = reinterpret_cast<uint64_t*>(rring + (size_t)G.ring_slots * G.rw);
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-  const int ngroups = (G.sx + F_B - 1) / F_B;
+  const int ngroups = (G.sx + F_B - 1) / F_B, SD = G.sd;
   // above every integer key / above every uint32 cost; low word above every raster index
   const unsigned long long kinit = ((unsigned long long)(SQ ? 0xffffffffu : FK_INIT_HI) << 32) | 0xffffffffu;
   if (tid == 0) { mbar_init(&bars[0], 1); mbar_init(&bars[1], 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
@@ -359,22 +379,32 @@ k1_fast_abs_kernel(const uint16_t* __restrict__ L16, const uint16_t* __restrict_
     const uint16_t* lsrc = L16 + ((size_t)strip * G.lrows + y0) * F_COLS;
     const uint16_t* rsrc = R16 + ((size_t)strip * G.rrows + y0 + dy0) * G.rw;
     if (tid == 0) {
+      // first period: right rows 0 .. ltile_rows + min(sd, ndy) - 2 -> slots 0.. (never past the chunk's last row)
+      const uint32_t rbytes0 = (uint32_t)(G.ltile_rows + min(SD, ndy) - 1) * rrow_bytes;
       fence_proxy_async();
-      mbar_expect_tx(&bars[0], lbytes + (uint32_t)G.ltile_rows * rrow_bytes);
+      mbar_expect_tx(&bars[0], lbytes + rbytes0);
       tma_load_1d(ltile, lsrc, lbytes, &bars[0]);
-      tma_load_1d(rring, rsrc, (uint32_t)G.ltile_rows * rrow_bytes, &bars[0]);     // right rows y0 .. y0+ltile_rows-1 -> slots 0..
+      tma_load_1d(rring, rsrc, rbytes0, &bars[0]);
     }
-    for (int k = tid; k < nrows * F_COLS; k += F_THREADS) { best[k] = (uint32_t)(kinit >> 32); keys[k] = kinit; }
+    for (int k = tid; k < nrows * F_COLS; k += FK_THREADS) { best[k] = (uint32_t)(kinit >> 32); keys[k] = kinit; }
     __syncthreads();
     mbar_wait(&bars[0], ph0); ph0 ^= 1;
-    for (int dy = 0; dy < ndy; ++dy) {         // dy relative to the chunk's first row dy0
-      const int ring_base = dy % G.ring_slots;
-      if (tid == 0 && dy + 1 < ndy) {        // prefetch the row iteration dy+1 adds, into the slot iteration dy-1 freed
+    for (int dyp = 0; dyp < ndy; dyp += SD) {      // periods of sd dy rows, relative to the chunk's first row dy0
+      const int dcur = min(SD, ndy - dyp);               // dy rows of this period
+      const int nnext = min(SD, ndy - dyp - dcur);       // dy rows of the next one: their last right rows are fetched now
+      if (tid == 0 && nnext > 0) {                       // into the slots the previous period freed
         fence_proxy_async();
-        mbar_expect_tx(&bars[1], rrow_bytes);
-        tma_load_1d(rring + (size_t)((dy + G.ltile_rows) % G.ring_slots) * G.rw, rsrc + (size_t)(dy + G.ltile_rows) * G.rw, rrow_bytes, &bars[1]);
+        mbar_expect_tx(&bars[1], (uint32_t)nnext * rrow_bytes);
+        for (int j = 0; j < nnext; ++j) {
+          const int rr = dyp + SD - 1 + G.ltile_rows + j;
+          tma_load_1d(rring + (size_t)(rr % G.ring_slots) * G.rw, rsrc + (size_t)rr * G.rw, rrow_bytes, &bars[1]);
+        }
       }
-      for (int g = w; g < ngroups; g += F_WARPS) {     // warp w: octets w, w+8, ... over all rows of the band
+      // units u = dl * ngroups + g of the period, dealt statically: warp w runs u = w, w + 12, ...  Warps on different dy
+      // of the period offer to the same key plane; the 64-bit atomicMin makes the result independent of their timing.
+      for (int u = w; u < dcur * ngroups; u += FK_WARPS) {
+        const int dy = dyp + u / ngroups, g = u % ngroups;
+        const int ring_base = dy % G.ring_slots;
         const int idx_base = (dy0 + dy) * G.sx + F_B * g;
         if (SQ) fast_pass_sq<KX>(ltile, rring, best, keys, lane, g, G.ky, G.ring_slots, G.rw, ring_base, idx_base, nrows, min(F_B, G.sx - F_B * g));
         else if (G.sx - F_B * g >= F_B)
@@ -382,12 +412,12 @@ k1_fast_abs_kernel(const uint16_t* __restrict__ L16, const uint16_t* __restrict_
         else
           fast_pass<KX, false>(ltile, rring, best, keys, lane, g, G.ky, G.ring_slots, G.rw, ring_base, idx_base, nrows, G.sx - F_B * g);
       }
-      if (dy + 1 < ndy) { mbar_wait(&bars[1], ph1); ph1 ^= 1; }
+      if (nnext > 0) { mbar_wait(&bars[1], ph1); ph1 ^= 1; }
       __syncthreads();
     }
     // ---- write {dx, dy, valid} (or this dy chunk's partial result) ----
     const int s0 = strip * G.out_cols;
-    for (int pix = tid; pix < nrows * G.out_cols; pix += F_THREADS) {
+    for (int pix = tid; pix < nrows * G.out_cols; pix += FK_THREADS) {
       const int x = pix % G.out_cols, y = pix / G.out_cols;
       const int gx = s0 + x, gy = y0 + y;
       if (gx >= G.W) continue;
@@ -486,7 +516,7 @@ int k1_fast_launch(int cost, ImgF left, ImgF right, int W, int H, int sx, int sy
   }
   VWB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FK_SMEM));   // per-function state shared by all host threads: device maximum
   if (ev && ev->e0) cudaEventRecord(ev->e0, st);
-  kern<<<grid, F_THREADS, smem, st>>>(L16, R16, g, out, opitch, part_cost, part_idx, gkeys);
+  kern<<<grid, FK_THREADS, smem, st>>>(L16, R16, g, out, opitch, part_cost, part_idx, gkeys);
   VWB_LAUNCH_CHECK();
   if (ev && ev->e1) cudaEventRecord(ev->e1, st);
   if (g.J > 1) {

@@ -18,13 +18,13 @@ struct FastGeom {
   int NS, NB;        // strips, bands
   int lrows, rrows;  // padded row counts of the packed arrays
   int ltile_rows;    // th + ky - 1
-  int ring_slots;    // th + ky
+  int ring_slots;    // th + ky; ltile_rows + 2*sd - 1 with periods of sd dy rows
   int rw;            // u16 per packed right row = 256 + sx (multiple of 8)
   int scale;                // values are packed as (v - vmin) * scale: 8 for AbsoluteCost (keys = cost*8+b), 1 for SquaredCost
   int J, dy_per;            // the dy range is split into J chunks of dy_per rows (more, smaller work items for small rasters)
   int lox, loy, rox, roy;   // origin of the (logical) left / right rasters inside the images passed to the pack kernels
   int addx, addy;           // constant added to the output disparities
-  int sd;                   // k1_screen: dy rows per synchronisation period (ring depth)
+  int sd;                   // dy rows per synchronisation period (ring depth)
   int th;                   // output rows per band (F_TH for k1_screen; k1_fast sizes it from its shared-memory budget)
 };
 static inline FastGeom make_geom(int W, int H, int sx, int sy, int kx, int ky, int th = F_TH) {
