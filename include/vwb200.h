@@ -114,6 +114,27 @@ int vwb200_disparity_mask(const vwb200_dispi* in, int w, int h,
                           vwb200_dispi* out, int on_device, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * The outlier filters of src/vw/Stereo/DisparityMap.h on integer or float disparities:
+ *   method THRESH, cleanup 0 / 1: rm_outliers_using_thresh / disparity_cleanup_using_thresh  (:318-442)
+ *   method MEAN,   cleanup 0 / 1: rm_outliers_using_mean   / disparity_cleanup_using_mean    (:444-598)
+ *   method STDDEV, cleanup 0 / 1: rm_outliers_using_stddev / disparity_cleanup_using_stddev  (:600-767)
+ * THRESH and STDDEV read pixel_threshold and rejection_threshold, MEAN reads max_mean_diff.  The cleanup composites add
+ * the reference's second RmOutliersUsingThreshFunc(1, 1, 3.0, 0.2) pass, which reads the first pass at the image's
+ * border without a second edge extension.  Each output pixel is computed from the input, so out must not overlap in
+ * (VWB200_EARG).  A rejected pixel becomes {0, 0, 0}; every other pixel is copied unchanged.  Results are bit for bit
+ * the reference's for finite disparities with |dx|, |dy| < 2^30.  rm_outliers_using_stddev uses every valid window pixel;
+ * the reference writes past its (2 * half_v + 1)^2 value vector when half_h > half_v and more pixels than that are valid.
+ * in / out: w x h pixels of pixel_type, row pitches in pixels.  half_h or half_v <= 0, an unknown method, cleanup or
+ * pixel type: VWB200_EARG.  A window whose tile and halo exceed the kernel's shared memory: VWB200_ENOIMPL.
+ * ------------------------------------------------------------------------------------------- */
+enum { VWB200_DISP_I32 = 0, VWB200_DISP_F32 = 1 };                 /* {int32 x3} / {float x3} pixels */
+enum { VWB200_OUTLIERS_THRESH = 0, VWB200_OUTLIERS_MEAN = 1, VWB200_OUTLIERS_STDDEV = 2 };
+typedef struct { int32_t method, cleanup, half_h, half_v;
+                 double pixel_threshold, rejection_threshold, max_mean_diff; } vwb200_outlier_params;
+int vwb200_outlier_filter(const vwb200_outlier_params* p, int pixel_type, const void* in, int w, int h, ptrdiff_t pitch,
+                          void* out, ptrdiff_t opitch, int on_device, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * vw::stereo::ParabolaSubpixelView::rasterize(dest, bbox) (src/vw/Stereo/ParabolaSubpixelView.h:27-117,
  * .cc:31-330): 3x3 AbsoluteCost patch around the integer disparity, 6x9 pseudo-inverse parabola fit,
  * offset kept when its norm is below 5.  disparity: cols x rows PixelMask<Vector2f> triples (same size as

@@ -7,6 +7,9 @@ Names, argument order and error behaviour follow Vision Workbench:
   * pyramid_correlate         -- src/vw/Stereo/CorrelationView.h:195-230
   * cross_corr_consistency_check, rm_outliers_using_thresh, disparity_cleanup_using_thresh,
     disparity_mask            -- src/vw/Stereo/Correlate.h:52-58, DisparityMap.h:318-442,97-253
+  * rm_outliers_using_mean, disparity_cleanup_using_mean, rm_outliers_using_stddev, disparity_cleanup_using_stddev
+    (int32 or float32 disparities; outlier_filter reaches all six filters on both)
+                              -- src/vw/Stereo/DisparityMap.h:444-767
   * disparity_median_filter, texture_measure, texture_preserving_disparity_filter
                               -- src/vw/Stereo/Algorithms.cc:26-67, Algorithms.h:144-281
 
@@ -118,6 +121,7 @@ def lib():
         L.vwb200_rm_outliers_using_thresh.argtypes = [P, I, I, I, I, D, D, P, I, P]
         L.vwb200_disparity_cleanup_using_thresh.argtypes = [P, I, I, I, I, D, D, P, I, P]
         L.vwb200_disparity_mask.argtypes = [P, I, I, P, P, I, I, P, I, P]
+        L.vwb200_outlier_filter.argtypes = [C.POINTER(OutlierParams), I, P, I, I, Z, P, Z, I, P]
         L.vwb200_corr_create.argtypes = [C.POINTER(CorrParams), C.POINTER(P)]
         L.vwb200_corr_set_inputs.argtypes = [P, P, I, I, Z, P, I, I, Z, P, Z, P, Z, I]
         L.vwb200_corr_rasterize.argtypes = [P, I, I, I, I, P, Z, I, P]
@@ -384,6 +388,62 @@ def disparity_mask(disparity_map, left_mask, right_mask):
     _check(lib().vwb200_disparity_mask(a.ctypes.data, a.shape[1], a.shape[0], lm.ctypes.data, rm.ctypes.data,
                                        rm.shape[1], rm.shape[0], out.ctypes.data, 0, None))
     return out
+
+
+class OutlierParams(C.Structure):
+    _fields_ = [("method", C.c_int32), ("cleanup", C.c_int32), ("half_h", C.c_int32), ("half_v", C.c_int32),
+                ("pixel_threshold", C.c_double), ("rejection_threshold", C.c_double), ("max_mean_diff", C.c_double)]
+
+
+# vwb200_outlier_filter's methods and pixel types (include/vwb200.h)
+OUTLIERS_THRESH, OUTLIERS_MEAN, OUTLIERS_STDDEV = 0, 1, 2
+DISP_I32, DISP_F32 = 0, 1
+
+
+def outlier_filter(method, cleanup, disparity_map, half_h, half_v, pixel_threshold=0.0, rejection_threshold=0.0, max_mean_diff=0.0):
+    """vwb200_outlier_filter: one of the six neighbourhood outlier filters of Stereo/DisparityMap.h on an int32
+    (PixelMask<Vector2i>) or float32 (PixelMask<Vector2f>) (rows, cols, 3) {dx, dy, valid} disparity, a numpy array or a
+    CUDA tensor on the current stream.  Returns a new array or tensor of the same type; the input is not changed."""
+    if _is_torch(disparity_map):
+        import torch
+        dt = {torch.int32: np.int32, torch.float32: np.float32}.get(disparity_map.dtype)
+    else:
+        dt = np.asarray(disparity_map).dtype.type
+    if dt not in (np.int32, np.float32) or len(disparity_map.shape) != 3 or disparity_map.shape[2] != 3:
+        raise ArgumentErr("the disparity must be an int32 or float32 (rows, cols, 3) array or CUDA tensor")
+    t, ptr, cols, rows, pitch, dev = _raster(disparity_map, dt, channels=3)
+    out = _output(t, (rows, cols, 3), dt)
+    p = OutlierParams(int(method), int(bool(cleanup)), int(half_h), int(half_v), float(pixel_threshold), float(rejection_threshold),
+                      float(max_mean_diff))
+    _check(lib().vwb200_outlier_filter(C.byref(p), DISP_I32 if dt == np.int32 else DISP_F32, ptr, cols, rows, pitch, _ptr(out), cols, dev,
+                                       _stream_ptr() if dev else None))
+    return out
+
+
+def rm_outliers_using_mean(disparity_map, half_h_kernel, half_v_kernel, max_mean_diff):
+    """rm_outliers_using_mean (Stereo/DisparityMap.h:444-578): a valid pixel further than max_mean_diff from the mean of
+    its window's valid pixels is rejected.  Pixels longer (|dx| + |dy|) than twice the window's 75th-percentile length end
+    their window row, as in the reference.  int32 or float32 (rows, cols, 3), numpy or CUDA; returns a new raster."""
+    return outlier_filter(OUTLIERS_MEAN, 0, disparity_map, half_h_kernel, half_v_kernel, max_mean_diff=max_mean_diff)
+
+
+def disparity_cleanup_using_mean(disparity_map, h_half_kernel, v_half_kernel, max_mean_diff):
+    """disparity_cleanup_using_mean (Stereo/DisparityMap.h:580-598): rm_outliers_using_mean, then the isolated-pixel pass
+    RmOutliersUsingThreshFunc(1, 1, 3.0, 0.2)."""
+    return outlier_filter(OUTLIERS_MEAN, 1, disparity_map, h_half_kernel, v_half_kernel, max_mean_diff=max_mean_diff)
+
+
+def rm_outliers_using_stddev(disparity_map, half_h_kernel, half_v_kernel, pixel_threshold, rejection_threshold):
+    """rm_outliers_using_stddev (Stereo/DisparityMap.h:600-748): a valid pixel further than pixel_threshold standard
+    deviations (at least rejection_threshold) from its window's mean, on either axis, is rejected.  int32 or float32
+    (rows, cols, 3), numpy or CUDA; returns a new raster."""
+    return outlier_filter(OUTLIERS_STDDEV, 0, disparity_map, half_h_kernel, half_v_kernel, pixel_threshold, rejection_threshold)
+
+
+def disparity_cleanup_using_stddev(disparity_map, h_half_kernel, v_half_kernel, pixel_threshold, rejection_threshold):
+    """disparity_cleanup_using_stddev (Stereo/DisparityMap.h:750-767): rm_outliers_using_stddev, then the isolated-pixel
+    pass RmOutliersUsingThreshFunc(1, 1, 3.0, 0.2)."""
+    return outlier_filter(OUTLIERS_STDDEV, 1, disparity_map, h_half_kernel, v_half_kernel, pixel_threshold, rejection_threshold)
 
 
 def _disparity_arg(disparity):

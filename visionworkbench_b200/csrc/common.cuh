@@ -61,7 +61,19 @@ struct Arena {
   }
 };
 
+// ---- order-preserving keys of floats (median select, outlier cutoff) -----------------------------
+// -0.0 sorts just below +0.0; NaN is outside the contract
+__device__ __forceinline__ unsigned fkey(float f) {
+  unsigned u = __float_as_uint(f);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float kfloat(unsigned k) {
+  return __uint_as_float((k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k);
+}
+
 // ---- image descriptors (device pointers) ------------------------------------------------------
+// float disparity pixel {dx, dy, valid} (PixelMask<Vector2f>); vwb200_dispi is the integer one
+struct DispF { float dx, dy, valid; };
 struct ImgF { const float* p; int w, h; ptrdiff_t pitch; };
 struct ImgB { const uint8_t* p; int w, h; ptrdiff_t pitch; };
 
@@ -172,6 +184,13 @@ int rm_outliers_launch(const vwb200_dispi* in, int w, int h, int hx, int hy, dou
                        int x0, int y0, int ow, int oh, vwb200_dispi* out, cudaStream_t st);
 // pass 2 (1,1,3.0,0.20) reading the padded pass-1 buffer (w+2)x(h+2)
 int cleanup_pass2_launch(const vwb200_dispi* p1, int w, int h, vwb200_dispi* out, cudaStream_t st);
+int cleanup_pass2_launch(const DispF* p1, int w, int h, DispF* out, cudaStream_t st);
+// pass 1 of rm_outliers_using_{thresh,mean,stddev} (method: VWB200_OUTLIERS_*) on either pixel type, evaluated over
+// [x0,x0+ow) x [y0,y0+oh) of the constant-edge-extended input (row pitch ipitch); out has row pitch opitch.
+// T = vwb200_dispi or DispF.
+template <class T>
+int outlier_pass1_launch(int method, const T* in, int w, int h, ptrdiff_t ipitch, int hx, int hy, double pt, double rt,
+                         double max_mean_diff, int x0, int y0, int ow, int oh, T* out, ptrdiff_t opitch, cudaStream_t st);
 int disparity_mask_launch(const vwb200_dispi* in, int w, int h, ImgB lmask, ImgB rmask, vwb200_dispi* out, cudaStream_t st);
 // out[i] = {dx+ax, dy+ay, valid} as float triples (CorrelationView.cc:880-884)
 int finalize_launch(const vwb200_dispi* in, int w, int h, int ax, int ay, float* out, ptrdiff_t opitch_px,

@@ -918,6 +918,46 @@ struct AbiCall {
   }
 };
 
+// ---- the outlier filters on either pixel type (Stereo/DisparityMap.h:318-767) ------------------------------------
+// in: device raster of w x h pixels, row pitch ip; out: dense w x h.  Integer thresh runs the level loop's chain itself;
+// the other five filters run pass 1 of their method, unpadded, or padded and followed by pass 2 as in outlier_filter_chain.
+template <class T>
+static int outlier_filter_run(const vwb200_outlier_params& p, const T* in, int w, int h, ptrdiff_t ip, T* out, Arena& ar, cudaStream_t st) {
+  if constexpr (std::is_same<T, vwb200_dispi>::value) {
+    if (p.method == VWB200_OUTLIERS_THRESH) {
+      if (ip != w) {                                     // the thresh kernel reads a dense raster
+        vwb200_dispi* d;
+        VWB_TRY(ar.alloc(&d, (size_t)w * h));
+        VWB_CUDA(cudaMemcpy2DAsync(d, (size_t)w * sizeof(T), in, (size_t)ip * sizeof(T), (size_t)w * sizeof(T), h, cudaMemcpyDeviceToDevice, st));
+        in = d;
+      }
+      return outlier_filter_chain(in, w, h, p.half_h, p.half_v, p.pixel_threshold, p.rejection_threshold, p.cleanup != 0, ImgB{}, ImgB{},
+                                  out, ar, st);
+    }
+  }
+  if (!p.cleanup)
+    return outlier_pass1_launch(p.method, in, w, h, ip, p.half_h, p.half_v, p.pixel_threshold, p.rejection_threshold, p.max_mean_diff,
+                                0, 0, w, h, out, (ptrdiff_t)w, st);
+  T* t1;
+  VWB_TRY(ar.alloc(&t1, (size_t)(w + 2) * (h + 2)));
+  VWB_TRY(outlier_pass1_launch(p.method, in, w, h, ip, p.half_h, p.half_v, p.pixel_threshold, p.rejection_threshold, p.max_mean_diff,
+                               -1, -1, w + 2, h + 2, t1, (ptrdiff_t)w + 2, st));
+  return cleanup_pass2_launch(t1, w, h, out, st);
+}
+// one vwb200_outlier_filter call: the input staged or used in place, the output written densely and copied back
+template <class T>
+static int outlier_filter_typed(const vwb200_outlier_params& p, const T* in, int w, int h, ptrdiff_t pitch, T* out, ptrdiff_t opitch,
+                                int on_device, void* stream) {
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
+  const T* din; ptrdiff_t dp;
+  VWB_TRY(c.in(in, w, h, pitch, on_device, &din, &dp));
+  T* dout; ptrdiff_t dop;
+  VWB_TRY(c.out(out, w, h, opitch, on_device, &dout, &dop, (const T*)nullptr, 0, /*dense=*/true));
+  VWB_TRY(outlier_filter_run(p, din, w, h, dp, dout, c.ar, c.st));
+  return c.finish();
+}
+
 // ---- disparity smoothing (Stereo/Algorithms.{h,cc}) ----------------------------------------------------------------
 // the two in-place filters: run the sweep over the disparity (staged through HBM when on the host), report a stall
 template <class Run>
@@ -1420,6 +1460,31 @@ int vwb200_disparity_cleanup_using_thresh(const vwb200_dispi* in, int w, int h, 
 int vwb200_disparity_mask(const vwb200_dispi* in, int w, int h, const uint8_t* lm, const uint8_t* rm, int rmw, int rmh, vwb200_dispi* out, int on_device, void* stream) {
   if (!lm || !rm) { set_error("disparity_mask: null mask"); return VWB200_EARG; }
   return filter_common(2, in, w, h, 1, 1, 0, 0, lm, rm, rmw, rmh, out, on_device, stream);
+}
+
+int vwb200_outlier_filter(const vwb200_outlier_params* p, int pixel_type, const void* in, int w, int h, ptrdiff_t pitch, void* out,
+                          ptrdiff_t opitch, int on_device, void* stream) {
+  if (!p || !in || !out) { set_error("outlier_filter: null pointer"); return VWB200_EARG; }
+  if (p->method < VWB200_OUTLIERS_THRESH || p->method > VWB200_OUTLIERS_STDDEV) { set_error("outlier_filter: unknown method %d", p->method); return VWB200_EARG; }
+  if (p->cleanup != 0 && p->cleanup != 1) { set_error("outlier_filter: cleanup must be 0 or 1, not %d", p->cleanup); return VWB200_EARG; }
+  if (pixel_type != VWB200_DISP_I32 && pixel_type != VWB200_DISP_F32) { set_error("outlier_filter: unknown pixel type %d", pixel_type); return VWB200_EARG; }
+  if (p->half_h <= 0 || p->half_v <= 0) {                // DisparityMap.h:343-344, :470-471, :631-632
+    set_error(p->method == VWB200_OUTLIERS_MEAN ? "RmOutliersUsingMeanFunc: half kernel sizes must be non-zero."
+                                                : "RmOutliersFunc: half kernel sizes must be non-zero.");
+    return VWB200_EARG;
+  }
+  if (w < 0 || h < 0 || pitch < w || opitch < w) { set_error("outlier_filter: bad size %d x %d, pitches %td, %td", w, h, pitch, opitch); return VWB200_EARG; }
+  if (w > 0 && h > 0) {                                  // each output pixel reads a window of the input: no overlap
+    const size_t px = 12;
+    const uintptr_t a0 = (uintptr_t)in, a1 = a0 + ((size_t)(h - 1) * pitch + w) * px;
+    const uintptr_t b0 = (uintptr_t)out, b1 = b0 + ((size_t)(h - 1) * opitch + w) * px;
+    if (a0 < b1 && b0 < a1) { set_error("outlier_filter: out overlaps in (the filters are not in place)"); return VWB200_EARG; }
+  }
+  VWB_TRY(ensure_device());
+  if (!w || !h) return VWB200_OK;
+  if (pixel_type == VWB200_DISP_I32)
+    return outlier_filter_typed(*p, (const vwb200_dispi*)in, w, h, pitch, (vwb200_dispi*)out, opitch, on_device, stream);
+  return outlier_filter_typed(*p, (const DispF*)in, w, h, pitch, (DispF*)out, opitch, on_device, stream);
 }
 
 // ---- the view -------------------------------------------------------------------------------------

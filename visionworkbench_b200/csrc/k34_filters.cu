@@ -128,32 +128,216 @@ int rm_outliers_launch(const vwb200_dispi* in, int w, int h, int hx, int hy, dou
   return VWB200_OK;
 }
 
+// The pixel types of the outlier filters: PixelMask<Vector2i> and PixelMask<Vector2f>, valid when valid != 0.  absdiff is
+// the reference's fabs((*acc)[0] - (*col_acc)[0]): the difference in the pixel type (int, or a rounded float), then a
+// double.  key is |dx| + |dy| in the pixel type (RmOutliersUsingMeanFunc's len, DisparityMap.h:504) as an order-preserving
+// uint32: the int itself, or the float's fkey (the sum is never negative); kval is the key's value as a double.
+template <class T> struct OutlierPx;
+template <> struct OutlierPx<vwb200_dispi> {
+  typedef int V;
+  static __device__ __forceinline__ bool valid(const vwb200_dispi& p) { return p.valid != 0; }
+  static __device__ __forceinline__ double absdiff(int a, int b) { return fabs((double)(a - b)); }
+  static __device__ __forceinline__ unsigned key(int dx, int dy) { return (unsigned)(abs(dx) + abs(dy)); }
+  static __device__ __forceinline__ double kval(unsigned k) { return (double)(int)k; }
+};
+template <> struct OutlierPx<DispF> {
+  typedef float V;
+  static __device__ __forceinline__ bool valid(const DispF& p) { return p.valid != 0.0f; }
+  static __device__ __forceinline__ double absdiff(float a, float b) { return (double)fabsf(__fsub_rn(a, b)); }
+  static __device__ __forceinline__ unsigned key(float dx, float dy) { return fkey(__fadd_rn(fabsf(dx), fabsf(dy))); }
+  static __device__ __forceinline__ double kval(unsigned k) { return (double)kfloat(k); }
+};
+
 // second pass (1,1,3.0,0.20) over the padded first-pass buffer p1 of size (w+2) x (h+2)  (DisparityMap.h:440)
-__global__ void cleanup_pass2_kernel(const vwb200_dispi* __restrict__ p1, int w, int h, vwb200_dispi* __restrict__ out) {
+template <class T>
+__global__ void cleanup_pass2_kernel(const T* __restrict__ p1, int w, int h, T* __restrict__ out) {
+  typedef OutlierPx<T> Px;
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
   if (x >= w || y >= h) return;
   const int pw = w + 2;
-  vwb200_dispi c = p1[(ptrdiff_t)(y + 1) * pw + (x + 1)];
-  if (c.valid) {
+  T c = p1[(ptrdiff_t)(y + 1) * pw + (x + 1)];
+  if (Px::valid(c)) {
     int matched = 0;
 #pragma unroll
     for (int yk = -1; yk <= 1; ++yk)
 #pragma unroll
       for (int xk = -1; xk <= 1; ++xk) {
-        const vwb200_dispi n = p1[(ptrdiff_t)(y + 1 + yk) * pw + (x + 1 + xk)];
-        if (n.valid && fabs((double)(c.dx - n.dx)) <= 3.0 && fabs((double)(c.dy - n.dy)) <= 3.0) ++matched;
+        const T n = p1[(ptrdiff_t)(y + 1 + yk) * pw + (x + 1 + xk)];
+        if (Px::valid(n) && Px::absdiff(c.dx, n.dx) <= 3.0 && Px::absdiff(c.dy, n.dy) <= 3.0) ++matched;
       }
     if (((double)matched / 9.0) < 0.20) { c.dx = 0; c.dy = 0; c.valid = 0; }
   }
   out[(ptrdiff_t)y * w + x] = c;
 }
-int cleanup_pass2_launch(const vwb200_dispi* p1, int w, int h, vwb200_dispi* out, cudaStream_t st) {
+template <class T>
+static int cleanup_pass2_launch_t(const T* p1, int w, int h, T* out, cudaStream_t st) {
   if (w <= 0 || h <= 0) return VWB200_OK;
   dim3 b(32, 8), g((w + 31) / 32, (h + 7) / 8);
-  cleanup_pass2_kernel<<<g, b, 0, st>>>(p1, w, h, out);
+  cleanup_pass2_kernel<T><<<g, b, 0, st>>>(p1, w, h, out);
   VWB_LAUNCH_CHECK();
   return VWB200_OK;
 }
+int cleanup_pass2_launch(const vwb200_dispi* p1, int w, int h, vwb200_dispi* out, cudaStream_t st) {
+  return cleanup_pass2_launch_t(p1, w, h, out, st);
+}
+int cleanup_pass2_launch(const DispF* p1, int w, int h, DispF* out, cudaStream_t st) {
+  return cleanup_pass2_launch_t(p1, w, h, out, st);
+}
+
+// ---- K4 on both pixel types: pass 1 of rm_outliers_using_thresh / _mean / _stddev ----------------------------------------
+// (DisparityMap.h:359-386, :484-553, :646-723).  One thread per output pixel over [x0,x0+ow) x [y0,y0+oh) of the
+// ConstantEdgeExtension of `in`, as rm_outliers_kernel does; the CTA stages its tile + halo in shared memory as {dx}, {dy}
+// and a key word: kNoKeyO for an invalid pixel, else |dx| + |dy| as a key (mean) or 0.  Every sum runs in the reference's
+// row-major order with explicitly rounded operations (no contraction).
+static constexpr unsigned kNoKeyO = 0xFFFFFFFFu;   // above every key of a finite |dx| + |dy|
+static constexpr size_t kOutlierSmemMax = 200 * 1024;
+
+template <class T, int M>
+__global__ void __launch_bounds__(RO_TW * RO_TH)
+outlier_pass1_kernel(const T* __restrict__ in, int w, int h, ptrdiff_t ipitch, int hx, int hy, double pt, double rt, double mdsq,
+                     int x0, int y0, int ow, int oh, T* __restrict__ out, ptrdiff_t opitch) {
+  typedef OutlierPx<T> Px;
+  typedef typename Px::V V;
+  extern __shared__ unsigned osm[];
+  const int sw = RO_TW + 2 * hx, sh = RO_TH + 2 * hy, sn = sw * sh;
+  V* sdx = reinterpret_cast<V*>(osm);
+  V* sdy = sdx + sn;
+  unsigned* skey = osm + 2 * sn;
+  const int bx = x0 + blockIdx.x * RO_TW, by = y0 + blockIdx.y * RO_TH;
+  for (int k = threadIdx.y * RO_TW + threadIdx.x; k < sn; k += RO_TW * RO_TH) {
+    const int sx = k % sw, sy = k / sw;
+    const T v = in[(ptrdiff_t)clampi3(by - hy + sy, 0, h - 1) * ipitch + clampi3(bx - hx + sx, 0, w - 1)];
+    sdx[k] = v.dx;
+    sdy[k] = v.dy;
+    skey[k] = !Px::valid(v) ? kNoKeyO : M == VWB200_OUTLIERS_MEAN ? Px::key(v.dx, v.dy) : 0u;
+  }
+  __syncthreads();
+  const int ox = blockIdx.x * RO_TW + threadIdx.x, oy = blockIdx.y * RO_TH + threadIdx.y;
+  if (ox >= ow || oy >= oh) return;
+  // the centre keeps all three values, also when invalid ("return *acc")
+  T c = in[(ptrdiff_t)clampi3(y0 + oy, 0, h - 1) * ipitch + clampi3(x0 + ox, 0, w - 1)];
+  if (Px::valid(c)) {
+    const int base = threadIdx.y * sw + threadIdx.x;      // window corner in the tile
+    bool reject;
+    if (M == VWB200_OUTLIERS_THRESH) {                    // :362-384
+      int matched = 0;
+      for (int yk = 0; yk <= 2 * hy; ++yk) {
+        const int r = base + yk * sw;
+        for (int xk = 0; xk <= 2 * hx; ++xk)
+          if (skey[r + xk] != kNoKeyO && Px::absdiff(c.dx, sdx[r + xk]) <= pt && Px::absdiff(c.dy, sdy[r + xk]) <= pt) ++matched;
+      }
+      reject = __ddiv_rn((double)matched, (double)((2 * hx + 1) * (2 * hy + 1))) < rt;
+    } else if (M == VWB200_OUTLIERS_MEAN) {               // :497-550
+      // cutoff = 2 * (the floor(0.75 n)-th smallest len): a bitwise select over the keys, from the highest bit in which the
+      // window's smallest and largest keys differ (MedianOp of k6_smoothing.cu, here within one thread)
+      unsigned n = 0, mn = kNoKeyO, mx = 0;
+      for (int yk = 0; yk <= 2 * hy; ++yk) {
+        const unsigned* kr = skey + base + yk * sw;
+        for (int xk = 0; xk <= 2 * hx; ++xk) {
+          const unsigned k = kr[xk];
+          if (k != kNoKeyO) { ++n; mn = min(mn, k); mx = max(mx, k); }
+        }
+      }
+      unsigned t = (unsigned)(int)__dmul_rn(0.75, (double)n), p = mn;
+      const int hb = mn == mx ? -1 : 31 - __clz(mn ^ mx);
+      if (hb >= 0) p = mn & ~((2u << hb) - 1u);
+      for (int b = hb; b >= 0; --b) {                     // kNoKeyO has every bit set: never counted
+        const unsigned lim = 1u << b;
+        unsigned cnt = 0;
+        for (int yk = 0; yk <= 2 * hy; ++yk) {
+          const unsigned* kr = skey + base + yk * sw;
+          for (int xk = 0; xk <= 2 * hx; ++xk) cnt += (kr[xk] ^ p) < lim;
+        }
+        if (t >= cnt) { t -= cnt; p |= lim; }
+      }
+      const double cutoff = __dmul_rn(2.0, Px::kval(p));
+      // `if (val > cutoff) continue;` skips col_acc.next_col(): the rest of that window row reads the same pixel, so the
+      // row ends there
+      unsigned matched = 0;
+      double mX = 0.0, mY = 0.0;
+      for (int yk = 0; yk <= 2 * hy; ++yk) {
+        const int r = base + yk * sw;
+        for (int xk = 0; xk <= 2 * hx; ++xk) {
+          const unsigned k = skey[r + xk];
+          if (k == kNoKeyO) continue;
+          if (Px::kval(k) > cutoff) break;
+          mX = __dadd_rn(mX, (double)sdx[r + xk]);
+          mY = __dadd_rn(mY, (double)sdy[r + xk]);
+          ++matched;
+        }
+      }
+      double esq = __dadd_rn(mdsq, 1.0);
+      if (matched > 0) {
+        mX = __ddiv_rn(mX, (double)matched);
+        mY = __ddiv_rn(mY, (double)matched);
+        const double ex = __dsub_rn((double)c.dx, mX), ey = __dsub_rn((double)c.dy, mY);
+        esq = __dadd_rn(__dmul_rn(ex, ex), __dmul_rn(ey, ey));
+      }
+      reject = esq > mdsq;
+    } else {                                              // :659-720
+      unsigned matched = 0;
+      double mX = 0.0, mY = 0.0;
+      for (int yk = 0; yk <= 2 * hy; ++yk) {
+        const int r = base + yk * sw;
+        for (int xk = 0; xk <= 2 * hx; ++xk)
+          if (skey[r + xk] != kNoKeyO) {
+            mX = __dadd_rn(mX, (double)sdx[r + xk]);
+            mY = __dadd_rn(mY, (double)sdy[r + xk]);
+            ++matched;
+          }
+      }
+      reject = matched == 0;
+      if (matched > 0) {
+        mX = __ddiv_rn(mX, (double)matched);
+        mY = __ddiv_rn(mY, (double)matched);
+        double sX = 0.0, sY = 0.0;
+        for (int yk = 0; yk <= 2 * hy; ++yk) {
+          const int r = base + yk * sw;
+          for (int xk = 0; xk <= 2 * hx; ++xk)
+            if (skey[r + xk] != kNoKeyO) {
+              const double dX = __dsub_rn((double)sdx[r + xk], mX), dY = __dsub_rn((double)sdy[r + xk], mY);
+              sX = __dadd_rn(sX, __dmul_rn(dX, dX));
+              sY = __dadd_rn(sY, __dmul_rn(dY, dY));
+            }
+        }
+        double sdX = __dsqrt_rn(__ddiv_rn(sX, (double)matched)), sdY = __dsqrt_rn(__ddiv_rn(sY, (double)matched));
+        if (sdX < rt) sdX = rt;
+        if (sdY < rt) sdY = rt;
+        const double eX = fabs(__dsub_rn((double)c.dx, mX)), eY = fabs(__dsub_rn((double)c.dy, mY));
+        reject = eX > __dmul_rn(pt, sdX) || eY > __dmul_rn(pt, sdY);
+      }
+    }
+    if (reject) { c.dx = 0; c.dy = 0; c.valid = 0; }
+  }
+  out[(ptrdiff_t)oy * opitch + ox] = c;
+}
+
+template <class T>
+int outlier_pass1_launch(int method, const T* in, int w, int h, ptrdiff_t ipitch, int hx, int hy, double pt, double rt,
+                         double max_mean_diff, int x0, int y0, int ow, int oh, T* out, ptrdiff_t opitch, cudaStream_t st) {
+  if (hx <= 0 || hy <= 0) {                               // DisparityMap.h:343-344, :470-471, :631-632
+    set_error(method == VWB200_OUTLIERS_MEAN ? "RmOutliersUsingMeanFunc: half kernel sizes must be non-zero."
+                                             : "RmOutliersFunc: half kernel sizes must be non-zero.");
+    return VWB200_EARG;
+  }
+  if (ow <= 0 || oh <= 0) return VWB200_OK;
+  const size_t smem = (size_t)(RO_TW + 2 * hx) * (RO_TH + 2 * hy) * 3 * sizeof(unsigned);
+  if (smem > kOutlierSmemMax) { set_error("outlier filter half kernel %dx%d too large", hx, hy); return VWB200_ENOIMPL; }
+  const dim3 b(RO_TW, RO_TH), g((ow + RO_TW - 1) / RO_TW, (oh + RO_TH - 1) / RO_TH);
+  if (g.y > 65535) { set_error("outlier filter: %d rows are above the supported %d", oh, 65535 * RO_TH); return VWB200_ENOIMPL; }
+  void (*kern)(const T*, int, int, ptrdiff_t, int, int, double, double, double, int, int, int, int, T*, ptrdiff_t) =
+      method == VWB200_OUTLIERS_THRESH ? outlier_pass1_kernel<T, VWB200_OUTLIERS_THRESH>
+      : method == VWB200_OUTLIERS_MEAN ? outlier_pass1_kernel<T, VWB200_OUTLIERS_MEAN>
+                                       : outlier_pass1_kernel<T, VWB200_OUTLIERS_STDDEV>;
+  VWB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  kern<<<g, b, smem, st>>>(in, w, h, ipitch, hx, hy, pt, rt, max_mean_diff * max_mean_diff, x0, y0, ow, oh, out, opitch);
+  VWB_LAUNCH_CHECK();
+  return VWB200_OK;
+}
+template int outlier_pass1_launch<vwb200_dispi>(int, const vwb200_dispi*, int, int, ptrdiff_t, int, int, double, double, double, int, int,
+                                                int, int, vwb200_dispi*, ptrdiff_t, cudaStream_t);
+template int outlier_pass1_launch<DispF>(int, const DispF*, int, int, ptrdiff_t, int, int, double, double, double, int, int, int, int,
+                                         DispF*, ptrdiff_t, cudaStream_t);
 
 // ---- disparity_mask (DisparityMap.h:142-162) --------------------------------------------------------------
 __global__ void disparity_mask_kernel(const vwb200_dispi* __restrict__ in, int w, int h, ImgB lm, ImgB rm, vwb200_dispi* __restrict__ out) {

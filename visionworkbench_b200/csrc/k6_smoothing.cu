@@ -40,15 +40,6 @@ __device__ __forceinline__ unsigned long long global_ns() {
   return t;
 }
 
-// order-preserving map of floats onto uint32 (-0.0 sorts just below +0.0; NaN is outside the contract)
-__device__ __forceinline__ unsigned fkey(float f) {
-  unsigned u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float kfloat(unsigned k) {
-  return __uint_as_float((k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k);
-}
-
 // sweep state: progress[row] = columns of the row completed; ticket; error word (1 = stalled)
 struct Sweep { int* progress; int* ticket; int* error; };
 
