@@ -135,6 +135,54 @@ int vwb200_outlier_filter(const vwb200_outlier_params* p, int pixel_type, const 
                           void* out, ptrdiff_t opitch, int on_device, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Resampling, range and transforms of a disparity image (src/vw/Stereo/DisparityMap.h) on either pixel type
+ * (VWB200_DISP_I32 / VWB200_DISP_F32); in / out are row-major, row pitches in pixels.  A pixel is valid when valid != 0.
+ * Pixels the engine creates get valid = 1 (or 1.0f), invalid ones {0, 0, 0} unless stated otherwise; pixels the reference
+ * passes through are copied unchanged, valid word included.  Results are bit for bit the reference's (floats as raw bits;
+ * NaN payloads are not kept) inside the value limits given per call.
+ *
+ * disparity_subsample (:1251-1322): out is (1 + (w-1)/2) x (1 + (h-1)/2).  The 10 / 5 / 2 weighted mean of the valid
+ * pixels of each 3 x 3 neighbourhood at stride 2, clamped reads at the border, summed in double (float pixels) or int64
+ * (int32 pixels, then truncating division) in the reference's order.  int32: |dx|, |dy| < 2^28 (the reference multiplies
+ * six of the nine terms in int32).  out must not overlap in.
+ * disparity_upsample (:1324-1358): out is 2w x 2h, each pixel child(x >> 1, y >> 1) * 2 with the child's validity (invalid
+ * pixels keep their doubled values and valid = 0).  int32: |dx|, |dy| < 2^30.  out must not overlap in.
+ * ------------------------------------------------------------------------------------------- */
+int vwb200_disparity_subsample(int pixel_type, const void* in, int w, int h, ptrdiff_t pitch, void* out, ptrdiff_t opitch,
+                               int on_device, void* stream);
+int vwb200_disparity_upsample(int pixel_type, const void* in, int w, int h, ptrdiff_t pitch, void* out, ptrdiff_t opitch,
+                              int on_device, void* stream);
+/* get_disparity_range (:48-66, PixelAccumulator<EWMinMaxAccumulator>, Image/Statistics.h:193-223): range (host, 4 floats)
+ * receives BBox2f(min, max) = {min dx, min dy, max dx, max dy} over the valid pixels in raster order, integers converted to
+ * float; (0, 0, 0, 0) when no pixel is valid.  Among equal values (-0.0 / +0.0) the first in raster order is kept; a NaN of
+ * the first valid pixel sticks, later NaNs are skipped.  any_valid (may be NULL) receives 1 or 0.  w * h < 2^32. */
+int vwb200_get_disparity_range(int pixel_type, const void* in, int w, int h, ptrdiff_t pitch, float* range, int* any_valid,
+                               int on_device, void* stream);
+/* disparity_range_mask (:255-300): min / max (host) point at two int32 or two floats, the children of the reference's
+ * min / max pixels.  A valid pixel with x + dx < min[0], x + dx >= max[0] - 1, y + dy < min[0] (sic, :279) or
+ * y + dy >= max[1] - 1 (in double; max - 1 in the channel type) becomes {0, 0, 0}; every other pixel is copied.
+ * out may be in (same pitch) but must not overlap it otherwise. */
+int vwb200_disparity_range_mask(int pixel_type, const void* in, int w, int h, ptrdiff_t pitch, const void* min, const void* max,
+                                void* out, ptrdiff_t opitch, int on_device, void* stream);
+/* transform_disparities.  matrix: the 3 x 3 matrix (row-major doubles) that is applied, p -> (m p) / w in homogeneous
+ * coordinates, in the order of HomographyTransform (Math/Transform.h:377-387).
+ *   VWB200_TRANSFORM_LAZY: transform_disparities(disparity, HomographyTransform(H)) (:1016-1057) with matrix = inverse(H),
+ *     the matrix HomographyTransform::reverse applies: out = m(loc + d) - loc.  Invalid pixels stay invalid (valid = 0)
+ *     and receive the transformed values.  do_round and the subregion are not used.
+ *   VWB200_TRANSFORM_EXPLICIT: transform_disparities(do_round, subregion, matrix, disparity) (:1190-1224) with
+ *     beg = subregion.min() + loc: out = m(beg + d) - beg, rounded half away from zero (std::round) when do_round.
+ *     Invalid pixels give {0, 0, 0}.  The subregion {x0, y0, x1, y1} must be w x h (VWB200_EARG, the reference's message).
+ * The matrix is applied as given; a singular one is not refused here (the C++ shim and the Python mirror refuse it as the
+ * reference's HomographyTransform constructor does).
+ * int32 pixels take the results truncated toward zero; a NaN or out-of-range result gives INT32_MIN, as x86-64 builds of the
+ * reference give (the C++ conversion is undefined there).
+ * out may be in (same pitch) but must not overlap it otherwise. */
+enum { VWB200_TRANSFORM_LAZY = 0, VWB200_TRANSFORM_EXPLICIT = 1 };
+int vwb200_transform_disparities(int pixel_type, int mode, const double* matrix, int do_round, const int32_t* subregion,
+                                 const void* in, int w, int h, ptrdiff_t pitch, void* out, ptrdiff_t opitch, int on_device,
+                                 void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * vw::stereo::ParabolaSubpixelView::rasterize(dest, bbox) (src/vw/Stereo/ParabolaSubpixelView.h:27-117,
  * .cc:31-330): 3x3 AbsoluteCost patch around the integer disparity, 6x9 pseudo-inverse parabola fit,
  * offset kept when its norm is below 5.  disparity: cols x rows PixelMask<Vector2f> triples (same size as

@@ -73,6 +73,39 @@ public:
   void expand(int32 o) { if (empty()) return; m_min[0] -= o; m_min[1] -= o; m_max[0] += o; m_max[1] += o; }
 };
 
+class BBox2f {                                                                          // Math/BBox.h: BBox(min, max)
+  Vector2f m_min, m_max;
+public:
+  BBox2f() {}
+  BBox2f(Vector2f const& mn, Vector2f const& mx) : m_min(mn), m_max(mx) {}
+  BBox2f(float x, float y, float w, float h) : m_min(x, y), m_max(x + w, y + h) {}
+  Vector2f const& min() const { return m_min; } Vector2f const& max() const { return m_max; }
+};
+
+// Math/Matrix.h: a fixed 3 x 3 matrix of doubles, row-major, m(row, col)
+struct Matrix3x3 {
+  double m[9];
+  Matrix3x3() { for (double& v : m) v = 0.0; }
+  double& operator()(size_t r, size_t c) { return m[3 * r + c]; }
+  double const& operator()(size_t r, size_t c) const { return m[3 * r + c]; }
+  size_t rows() const { return 3; } size_t cols() const { return 3; }
+  void set_identity() { for (int i = 0; i < 9; ++i) m[i] = (i % 4 == 0) ? 1.0 : 0.0; }
+};
+namespace math {
+// vw::math::inverse (Math/Matrix.h:2218-2270, LU decomposition with partial pivoting in the reference): here the adjugate over
+// the determinant, which agrees with it to rounding, not bit for bit; a singular matrix throws MathErr as there
+inline Matrix3x3 inverse(Matrix3x3 const& a) {
+  Matrix3x3 r;
+  r(0, 0) = a(1, 1) * a(2, 2) - a(1, 2) * a(2, 1); r(0, 1) = a(0, 2) * a(2, 1) - a(0, 1) * a(2, 2); r(0, 2) = a(0, 1) * a(1, 2) - a(0, 2) * a(1, 1);
+  r(1, 0) = a(1, 2) * a(2, 0) - a(1, 0) * a(2, 2); r(1, 1) = a(0, 0) * a(2, 2) - a(0, 2) * a(2, 0); r(1, 2) = a(0, 2) * a(1, 0) - a(0, 0) * a(1, 2);
+  r(2, 0) = a(1, 0) * a(2, 1) - a(1, 1) * a(2, 0); r(2, 1) = a(0, 1) * a(2, 0) - a(0, 0) * a(2, 1); r(2, 2) = a(0, 0) * a(1, 1) - a(0, 1) * a(1, 0);
+  const double det = a(0, 0) * r(0, 0) + a(0, 1) * r(1, 0) + a(0, 2) * r(2, 0);
+  if (det == 0.0) vw_throw(MathErr() << "Matrix is singular in inverse()");
+  for (double& v : r.m) v /= det;
+  return r;
+}
+}  // namespace math
+
 // ---- pixels -----------------------------------------------------------------------------------------
 template <class T> struct PixelGray { T v; PixelGray() : v() {} PixelGray(T a) : v(a) {} operator T() const { return v; } };
 template <class ChildT> struct PixelMaskChannel;

@@ -12,6 +12,9 @@ Names, argument order and error behaviour follow Vision Workbench:
                               -- src/vw/Stereo/DisparityMap.h:444-767
   * disparity_median_filter, texture_measure, texture_preserving_disparity_filter
                               -- src/vw/Stereo/Algorithms.cc:26-67, Algorithms.h:144-281
+  * disparity_subsample, disparity_upsample, get_disparity_range, disparity_range_mask, transform_disparities,
+    transform_disparities_explicit (int32 or float32 disparities)
+                              -- src/vw/Stereo/DisparityMap.h:48-66, 255-300, 1016-1057, 1190-1224, 1251-1358
 
 There is no CPU path: every call goes to libvwb200.so (hand-written sm_90a kernels) and raises if
 the library or a CUDA device is missing.  Inputs may be numpy arrays (staged through HBM by the
@@ -122,6 +125,11 @@ def lib():
         L.vwb200_disparity_cleanup_using_thresh.argtypes = [P, I, I, I, I, D, D, P, I, P]
         L.vwb200_disparity_mask.argtypes = [P, I, I, P, P, I, I, P, I, P]
         L.vwb200_outlier_filter.argtypes = [C.POINTER(OutlierParams), I, P, I, I, Z, P, Z, I, P]
+        L.vwb200_disparity_subsample.argtypes = [I, P, I, I, Z, P, Z, I, P]
+        L.vwb200_disparity_upsample.argtypes = [I, P, I, I, Z, P, Z, I, P]
+        L.vwb200_get_disparity_range.argtypes = [I, P, I, I, Z, P, P, I, P]
+        L.vwb200_disparity_range_mask.argtypes = [I, P, I, I, Z, P, P, P, Z, I, P]
+        L.vwb200_transform_disparities.argtypes = [I, I, P, I, P, P, I, I, Z, P, Z, I, P]
         L.vwb200_corr_create.argtypes = [C.POINTER(CorrParams), C.POINTER(P)]
         L.vwb200_corr_set_inputs.argtypes = [P, P, I, I, Z, P, I, I, Z, P, Z, P, Z, I]
         L.vwb200_corr_rasterize.argtypes = [P, I, I, I, I, P, Z, I, P]
@@ -444,6 +452,117 @@ def disparity_cleanup_using_stddev(disparity_map, h_half_kernel, v_half_kernel, 
     """disparity_cleanup_using_stddev (Stereo/DisparityMap.h:750-767): rm_outliers_using_stddev, then the isolated-pixel
     pass RmOutliersUsingThreshFunc(1, 1, 3.0, 0.2)."""
     return outlier_filter(OUTLIERS_STDDEV, 1, disparity_map, h_half_kernel, v_half_kernel, pixel_threshold, rejection_threshold)
+
+
+# vwb200_transform_disparities' modes (include/vwb200.h)
+TRANSFORM_LAZY, TRANSFORM_EXPLICIT = 0, 1
+
+
+def _disparity_in(disparity_map):
+    """(keep-alive, pointer, cols, rows, pitch in pixels, on_device, numpy dtype) of an int32 or float32 (rows, cols, 3)
+    disparity, a numpy array or a CUDA tensor"""
+    if _is_torch(disparity_map):
+        import torch
+        dt = {torch.int32: np.int32, torch.float32: np.float32}.get(disparity_map.dtype)
+    else:
+        dt = np.asarray(disparity_map).dtype.type
+    if dt not in (np.int32, np.float32) or len(disparity_map.shape) != 3 or disparity_map.shape[2] != 3:
+        raise ArgumentErr("the disparity must be an int32 or float32 (rows, cols, 3) array or CUDA tensor")
+    return _raster(disparity_map, dt, channels=3) + (dt,)
+
+
+def _ptype(dt):
+    return DISP_I32 if dt == np.int32 else DISP_F32
+
+
+def disparity_subsample(disparity_map):
+    """disparity_subsample (Stereo/DisparityMap.h:1251-1322): the 10 / 5 / 2 weighted mean of the valid pixels of each
+    3 x 3 neighbourhood at stride 2 (clamped at the border), an image of 1 + (cols-1)/2 x 1 + (rows-1)/2 pixels.  int32 or
+    float32 (rows, cols, 3), numpy or CUDA; returns a new raster of the same kind."""
+    t, ptr, cols, rows, pitch, dev, dt = _disparity_in(disparity_map)
+    ow, oh = (1 + (cols - 1) // 2, 1 + (rows - 1) // 2) if cols and rows else (0, 0)
+    out = _output(t, (oh, ow, 3), dt)
+    _check(lib().vwb200_disparity_subsample(_ptype(dt), ptr, cols, rows, pitch, _ptr(out), ow, dev, _stream_ptr() if dev else None))
+    return out
+
+
+def disparity_upsample(disparity_map):
+    """disparity_upsample (Stereo/DisparityMap.h:1324-1358): each pixel doubled into a 2 x 2 block of a 2 cols x 2 rows
+    image, validity carried from the pixel.  int32 or float32 (rows, cols, 3), numpy or CUDA; returns a new raster."""
+    t, ptr, cols, rows, pitch, dev, dt = _disparity_in(disparity_map)
+    out = _output(t, (2 * rows, 2 * cols, 3), dt)
+    _check(lib().vwb200_disparity_upsample(_ptype(dt), ptr, cols, rows, pitch, _ptr(out), 2 * cols, dev, _stream_ptr() if dev else None))
+    return out
+
+
+def get_disparity_range(disparity_map):
+    """get_disparity_range (Stereo/DisparityMap.h:48-66): BBox2f(min, max) of the valid pixels' children as a BBox2f-like
+    tuple (min dx, min dy, max dx, max dy) of Python floats holding float32 values; (0, 0, 0, 0) without a valid pixel."""
+    t, ptr, cols, rows, pitch, dev, dt = _disparity_in(disparity_map)
+    r = (C.c_float * 4)()
+    _check(lib().vwb200_get_disparity_range(_ptype(dt), ptr, cols, rows, pitch, r, None, dev, _stream_ptr() if dev else None))
+    return tuple(r)
+
+
+def _pixel_out(t, rows, cols, dt, out):
+    if out is None:
+        return _output(t, (rows, cols, 3), dt), cols
+    if out is not t:
+        raise ArgumentErr("out must be None or the disparity itself")
+    return out, cols
+
+
+def disparity_range_mask(disparity_map, min, max, out=None):
+    """disparity_range_mask (Stereo/DisparityMap.h:255-300): a valid pixel that points outside [min, max - 1) of the
+    secondary image becomes {0, 0, 0} (the y coordinate is compared against min[0], as in the reference).  min / max: the
+    (dx, dy) children of the reference's min / max pixels.  out=None gives a new raster; out=disparity_map writes it in
+    place (a CUDA tensor or a C-contiguous numpy array)."""
+    t, ptr, cols, rows, pitch, dev, dt = _disparity_in(disparity_map)
+    o, op = _pixel_out(t, rows, cols, dt, out)
+    mn, mx = np.asarray(min, dt).reshape(2).copy(), np.asarray(max, dt).reshape(2).copy()
+    _check(lib().vwb200_disparity_range_mask(_ptype(dt), ptr, cols, rows, pitch, mn.ctypes.data, mx.ctypes.data, _ptr(o), pitch if out is not None else op,
+                                             dev, _stream_ptr() if dev else None))
+    return o
+
+
+def _homography(matrix):
+    """the 3 x 3 float64 matrix and its inverse, refused as HomographyTransform's constructor refuses it (Math/Matrix.h)"""
+    m = np.asarray(matrix, np.float64)
+    if m.shape != (3, 3):
+        raise ArgumentErr("Matrix must have dimensions 3x3.")
+    try:
+        return m, np.linalg.inv(m)
+    except np.linalg.LinAlgError:
+        raise MathErr("Matrix is singular in inverse()") from None
+
+
+def transform_disparities(disparity_map, homography, out=None):
+    """transform_disparities(disparity, HomographyTransform(H)) (Stereo/DisparityMap.h:1016-1057): each pixel becomes
+    reverse(loc + d) - loc with reverse() applying inverse(H), computed here with numpy; it agrees with vw::math::inverse to
+    rounding (pass the reference's inverse to vwb200_transform_disparities for its exact matrix).  Invalid pixels stay invalid
+    and receive the transformed values.  out: as in disparity_range_mask."""
+    return _transform(TRANSFORM_LAZY, _homography(homography)[1], False, None, disparity_map, out)
+
+
+def transform_disparities_explicit(do_round, subregion, T, disparity, out=None):
+    """transform_disparities(do_round, subregion, T, disparity) (Stereo/DisparityMap.h:1190-1224): each valid pixel becomes
+    T(beg + d) - beg with beg = subregion.min() + loc, rounded when do_round; invalid pixels give {0, 0, 0}.  subregion:
+    (x0, y0, x1, y1) or a BBox2i of the disparity's size (ArgumentErr otherwise).  T must be 3 x 3 (ArgumentErr) and
+    invertible (MathErr), as for the reference's HomographyTransform(T)."""
+    b = (subregion.x0, subregion.y0, subregion.x1, subregion.y1) if isinstance(subregion, BBox2i) else tuple(subregion)
+    if len(disparity.shape) == 3 and (b[2] - b[0] != disparity.shape[1] or b[3] - b[1] != disparity.shape[0]):   # checked first, as there
+        raise ArgumentErr("transform_disparities: The sizes of subregion and disparity don't match.\n")
+    return _transform(TRANSFORM_EXPLICIT, _homography(T)[0], do_round, b, disparity, out)
+
+
+def _transform(mode, matrix, do_round, box, disparity_map, out):
+    t, ptr, cols, rows, pitch, dev, dt = _disparity_in(disparity_map)
+    o, op = _pixel_out(t, rows, cols, dt, out)
+    m = np.ascontiguousarray(np.asarray(matrix, np.float64).reshape(9))
+    sub = (C.c_int32 * 4)(*[int(v) for v in box]) if box is not None else None
+    _check(lib().vwb200_transform_disparities(_ptype(dt), mode, m.ctypes.data, int(bool(do_round)), sub, ptr, cols, rows, pitch, _ptr(o),
+                                              pitch if out is not None else op, dev, _stream_ptr() if dev else None))
+    return o
 
 
 def _disparity_arg(disparity):

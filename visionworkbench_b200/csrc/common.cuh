@@ -212,6 +212,18 @@ int texture_filter_sweep_launch(float* d, int W, int H, ptrdiff_t pitch, const f
                                 int max_kernel_size, int* work, int* err_host, cudaStream_t st);
 int texture_measure_launch(ImgF img, int kernel_size, double gw, double sw, float* out, ptrdiff_t opitch, cudaStream_t st);
 
+// ---- K7: disparity resampling, range and transforms (k7_dispmap.cu); T = vwb200_dispi or DispF, pitches in pixels ----------
+// subsample: out is (1 + (w-1)/2) x (1 + (h-1)/2); upsample: out is 2w x 2h
+template <class T> int dispmap_subsample_launch(const T* in, int w, int h, ptrdiff_t ip, T* out, ptrdiff_t op, cudaStream_t st);
+template <class T> int dispmap_upsample_launch(const T* in, int w, int h, ptrdiff_t ip, T* out, ptrdiff_t op, cudaStream_t st);
+// keys5: 5 x 8 bytes of device scratch; res5 (device): min x, min y, max x, max y, any valid pixel (1 / 0); w * h < 2^32
+template <class T> int dispmap_range_launch(const T* in, int w, int h, ptrdiff_t ip, unsigned long long* keys5, float* res5, cudaStream_t st);
+// min2 / max2: host pointers to two channel values each; out may be in (same pitch)
+template <class T> int dispmap_range_mask_launch(const T* in, int w, int h, ptrdiff_t ip, const void* min2, const void* max2, T* out,
+                                                 ptrdiff_t op, cudaStream_t st);
+template <class T> int dispmap_transform_launch(int mode, const double* m9, int do_round, int sx0, int sy0, const T* in, int w, int h,
+                                                ptrdiff_t ip, T* out, ptrdiff_t op, cudaStream_t st);
+
 // ---- host-side restatement-free logic -----------------------------------------------------------
 struct Box { int x0, y0, x1, y1; };
 struct HostZone { Box img; Box disp; };

@@ -958,6 +958,61 @@ static int outlier_filter_typed(const vwb200_outlier_params& p, const T* in, int
   return c.finish();
 }
 
+// ---- K7: resampling, range and transforms of a disparity (Stereo/DisparityMap.h) ----------------------------------------------
+// the argument checks every K7 call shares; `what` names the call in the messages
+static int dispmap_check(const char* what, int pixel_type, const void* in, int w, int h, ptrdiff_t pitch) {
+  if (!in) { set_error("%s: null input", what); return VWB200_EARG; }
+  if (pixel_type != VWB200_DISP_I32 && pixel_type != VWB200_DISP_F32) { set_error("%s: unknown pixel type %d", what, pixel_type); return VWB200_EARG; }
+  if (w < 0 || h < 0 || pitch < w) { set_error("%s: bad size %d x %d, pitch %td", what, w, h, pitch); return VWB200_EARG; }
+  return VWB200_OK;
+}
+// [a0, a1) and [b0, b1): the bytes of an w x h / ow x oh raster of 12-byte pixels
+static bool rasters_overlap(const void* a, int w, int h, ptrdiff_t ap, const void* b, int ow, int oh, ptrdiff_t bp) {
+  if (w <= 0 || h <= 0 || ow <= 0 || oh <= 0) return false;
+  const uintptr_t a0 = (uintptr_t)a, a1 = a0 + ((size_t)(h - 1) * ap + w) * 12;
+  const uintptr_t b0 = (uintptr_t)b, b1 = b0 + ((size_t)(oh - 1) * bp + ow) * 12;
+  return a0 < b1 && b0 < a1;
+}
+// one resampling or per-pixel call: in (w x h) -> out (ow x oh), both staged through AbiCall.  launch(din, dp, dout, dop, st)
+// is called with device pointers of the pixel type; out == in on the device (same pitch) is used in place.
+template <class T, class Launch>
+static int dispmap_typed(const T* in, int w, int h, ptrdiff_t pitch, T* out, int ow, int oh, ptrdiff_t opitch, int on_device, void* stream,
+                         Launch launch) {
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
+  const T* din; ptrdiff_t dp;
+  VWB_TRY(c.in(in, w, h, pitch, on_device, &din, &dp));
+  T* dout; ptrdiff_t dop;
+  VWB_TRY(c.out(out, ow, oh, opitch, on_device, &dout, &dop));
+  VWB_TRY(launch(din, dp, dout, dop, c.st));
+  return c.finish();
+}
+template <class Launch>
+static int dispmap_run(int pixel_type, const void* in, int w, int h, ptrdiff_t pitch, void* out, int ow, int oh, ptrdiff_t opitch,
+                       int on_device, void* stream, Launch launch) {
+  if (pixel_type == VWB200_DISP_I32)
+    return dispmap_typed((const vwb200_dispi*)in, w, h, pitch, (vwb200_dispi*)out, ow, oh, opitch, on_device, stream, launch);
+  return dispmap_typed((const DispF*)in, w, h, pitch, (DispF*)out, ow, oh, opitch, on_device, stream, launch);
+}
+template <class T>
+static int dispmap_range_typed(const T* in, int w, int h, ptrdiff_t pitch, float* range, int* any_valid, int on_device, void* stream) {
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
+  const T* din; ptrdiff_t dp;
+  VWB_TRY(c.in(in, w, h, pitch, on_device, &din, &dp));
+  unsigned long long* keys;
+  float* res;
+  VWB_TRY(c.ar.alloc(&keys, 5));
+  VWB_TRY(c.ar.alloc(&res, 5));
+  VWB_TRY(dispmap_range_launch(din, w, h, dp, keys, res, c.st));
+  float r5[5];
+  VWB_CUDA(cudaMemcpyAsync(r5, res, sizeof(r5), cudaMemcpyDeviceToHost, c.st));
+  VWB_TRY(c.finish());
+  for (int i = 0; i < 4; ++i) range[i] = r5[i];
+  if (any_valid) *any_valid = r5[4] != 0.0f;
+  return VWB200_OK;
+}
+
 // ---- disparity smoothing (Stereo/Algorithms.{h,cc}) ----------------------------------------------------------------
 // the two in-place filters: run the sweep over the disparity (staged through HBM when on the host), report a stall
 template <class Run>
@@ -1485,6 +1540,97 @@ int vwb200_outlier_filter(const vwb200_outlier_params* p, int pixel_type, const 
   if (pixel_type == VWB200_DISP_I32)
     return outlier_filter_typed(*p, (const vwb200_dispi*)in, w, h, pitch, (vwb200_dispi*)out, opitch, on_device, stream);
   return outlier_filter_typed(*p, (const DispF*)in, w, h, pitch, (DispF*)out, opitch, on_device, stream);
+}
+
+// ---- K7 (Stereo/DisparityMap.h) -------------------------------------------------------------------------------------------
+static int dispmap_resample(bool up, int pixel_type, const void* in, int w, int h, ptrdiff_t pitch, void* out, ptrdiff_t opitch,
+                            int on_device, void* stream) {
+  const char* what = up ? "disparity_upsample" : "disparity_subsample";
+  VWB_TRY(dispmap_check(what, pixel_type, in, w, h, pitch));
+  if (!out) { set_error("%s: null output", what); return VWB200_EARG; }
+  if (up && ((long long)w * 2 > INT_MAX || (long long)h * 2 > INT_MAX)) { set_error("%s: %d x %d is too large", what, w, h); return VWB200_EARG; }
+  const int ow = up ? 2 * w : (w ? 1 + (w - 1) / 2 : 0), oh = up ? 2 * h : (h ? 1 + (h - 1) / 2 : 0);
+  if (opitch < ow) { set_error("%s: output pitch %td below its width %d", what, opitch, ow); return VWB200_EARG; }
+  if (rasters_overlap(in, w, h, pitch, out, ow, oh, opitch)) { set_error("%s: out overlaps in", what); return VWB200_EARG; }
+  VWB_TRY(ensure_device());
+  if (!w || !h) return VWB200_OK;
+  return dispmap_run(pixel_type, in, w, h, pitch, out, ow, oh, opitch, on_device, stream,
+                     [&](auto* din, ptrdiff_t dp, auto* dout, ptrdiff_t dop, cudaStream_t st) {
+                       return up ? dispmap_upsample_launch(din, w, h, dp, dout, dop, st) : dispmap_subsample_launch(din, w, h, dp, dout, dop, st);
+                     });
+}
+int vwb200_disparity_subsample(int pixel_type, const void* in, int w, int h, ptrdiff_t pitch, void* out, ptrdiff_t opitch, int on_device,
+                               void* stream) {
+  return dispmap_resample(false, pixel_type, in, w, h, pitch, out, opitch, on_device, stream);
+}
+int vwb200_disparity_upsample(int pixel_type, const void* in, int w, int h, ptrdiff_t pitch, void* out, ptrdiff_t opitch, int on_device,
+                              void* stream) {
+  return dispmap_resample(true, pixel_type, in, w, h, pitch, out, opitch, on_device, stream);
+}
+
+int vwb200_get_disparity_range(int pixel_type, const void* in, int w, int h, ptrdiff_t pitch, float* range, int* any_valid, int on_device,
+                               void* stream) {
+  VWB_TRY(dispmap_check("get_disparity_range", pixel_type, in, w, h, pitch));
+  if (!range) { set_error("get_disparity_range: null range"); return VWB200_EARG; }
+  if ((unsigned long long)w * (unsigned long long)h > 0xFFFFFFFFull) {
+    set_error("get_disparity_range: %d x %d pixels exceed the 2^32 raster indices of the reduction", w, h);
+    return VWB200_ENOIMPL;
+  }
+  VWB_TRY(ensure_device());
+  if (!w || !h) {                                                    // no pixel: BBox2f(0, 0, 0, 0)
+    range[0] = range[1] = range[2] = range[3] = 0.0f;
+    if (any_valid) *any_valid = 0;
+    return VWB200_OK;
+  }
+  if (pixel_type == VWB200_DISP_I32) return dispmap_range_typed((const vwb200_dispi*)in, w, h, pitch, range, any_valid, on_device, stream);
+  return dispmap_range_typed((const DispF*)in, w, h, pitch, range, any_valid, on_device, stream);
+}
+
+// the per-pixel calls: out may be in itself, with the same pitch, but may not overlap it otherwise
+static int dispmap_pixel_check(const char* what, int pixel_type, const void* in, int w, int h, ptrdiff_t pitch, const void* out, ptrdiff_t opitch) {
+  VWB_TRY(dispmap_check(what, pixel_type, in, w, h, pitch));
+  if (!out) { set_error("%s: null output", what); return VWB200_EARG; }
+  if (opitch < w) { set_error("%s: output pitch %td below the width %d", what, opitch, w); return VWB200_EARG; }
+  if (!(out == in && opitch == pitch) && rasters_overlap(in, w, h, pitch, out, w, h, opitch)) {
+    set_error("%s: out overlaps in (only out == in with the same pitch is allowed)", what);
+    return VWB200_EARG;
+  }
+  return VWB200_OK;
+}
+
+int vwb200_disparity_range_mask(int pixel_type, const void* in, int w, int h, ptrdiff_t pitch, const void* min, const void* max, void* out,
+                                ptrdiff_t opitch, int on_device, void* stream) {
+  VWB_TRY(dispmap_pixel_check("disparity_range_mask", pixel_type, in, w, h, pitch, out, opitch));
+  if (!min || !max) { set_error("disparity_range_mask: null min or max"); return VWB200_EARG; }
+  VWB_TRY(ensure_device());
+  if (!w || !h) return VWB200_OK;
+  return dispmap_run(pixel_type, in, w, h, pitch, out, w, h, opitch, on_device, stream,
+                     [&](auto* din, ptrdiff_t dp, auto* dout, ptrdiff_t dop, cudaStream_t st) {
+                       return dispmap_range_mask_launch(din, w, h, dp, min, max, dout, dop, st);
+                     });
+}
+
+int vwb200_transform_disparities(int pixel_type, int mode, const double* matrix, int do_round, const int32_t* subregion, const void* in,
+                                 int w, int h, ptrdiff_t pitch, void* out, ptrdiff_t opitch, int on_device, void* stream) {
+  VWB_TRY(dispmap_pixel_check("transform_disparities", pixel_type, in, w, h, pitch, out, opitch));
+  if (!matrix) { set_error("transform_disparities: null matrix"); return VWB200_EARG; }
+  if (mode != VWB200_TRANSFORM_LAZY && mode != VWB200_TRANSFORM_EXPLICIT) { set_error("transform_disparities: unknown mode %d", mode); return VWB200_EARG; }
+  int sx0 = 0, sy0 = 0;
+  if (mode == VWB200_TRANSFORM_EXPLICIT) {
+    if (!subregion) { set_error("transform_disparities: null subregion"); return VWB200_EARG; }
+    // BBox2i::width() / height(): max - min (DisparityMap.h:1197-1200)
+    if ((long long)subregion[2] - subregion[0] != w || (long long)subregion[3] - subregion[1] != h) {
+      set_error("transform_disparities: The sizes of subregion and disparity don't match.\n");
+      return VWB200_EARG;
+    }
+    sx0 = subregion[0]; sy0 = subregion[1];
+  }
+  VWB_TRY(ensure_device());
+  if (!w || !h) return VWB200_OK;
+  return dispmap_run(pixel_type, in, w, h, pitch, out, w, h, opitch, on_device, stream,
+                     [&](auto* din, ptrdiff_t dp, auto* dout, ptrdiff_t dop, cudaStream_t st) {
+                       return dispmap_transform_launch(mode, matrix, do_round != 0, sx0, sy0, din, w, h, dp, dout, dop, st);
+                     });
 }
 
 // ---- the view -------------------------------------------------------------------------------------
