@@ -183,6 +183,34 @@ int vwb200_transform_disparities(int pixel_type, int mode, const double* matrix,
                                  void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * transform(image, tx, edge, interp) (src/vw/Image/Transform.h:485-601) of a float image (PixelGray<float>), rasterised over
+ * the output window (x0, y0, ow, oh): out pixel (i, j) is the TransformView pixel (x0 + i, y0 + j).  The plain form is the
+ * window (0, 0, w, h), the width / height form (0, 0, width, height), the bbox form the bbox itself.
+ *   kind VWB200_WARP_HOMOGRAPHY: HomographyTransform(H) (Math/Transform.h:369-389); matrix is the 3 x 3 matrix (row-major
+ *     doubles) that reverse() applies, i.e. inverse(H), as VWB200_TRANSFORM_LAZY takes it.  The disparity is not used.
+ *   kind VWB200_WARP_DISPARITY: DisparityTransform(disparity) (Stereo/DisparityMap.h:1164-1187) on a dw x dh float
+ *     disparity ({dx, dy, valid} pixels, row pitch dpitch in pixels).  reverse(p) is p + (dx, dy) in double for a valid
+ *     pixel at p, and (-1, p.y) for an invalid one or a p outside the disparity.  The matrix is not used.
+ *   interp: VWB200_INTERP_BILINEAR (in float, Image/Interpolation.h:76-110), _BICUBIC (in double, :138-186) or _NEAREST
+ *     (math::impl::_round, ties away from zero, :209-225).  Bilinear and bicubic return the pixel itself when the reversed
+ *     point is integral, so NaN neighbours do not leak in there.
+ *   edge: VWB200_EDGE_ZERO (+0.0f outside the image) or VWB200_EDGE_CONSTANT (each axis clamped) (Image/EdgeExtension.tcc).
+ * Exactness: every pixel is bit for bit the reference's (floats as raw bits, NaN payloads not kept) when both reversed
+ * coordinates are finite with |c| < 2^30.  Elsewhere (including w == 0 of a homography inside the window, giving inf or NaN)
+ * the reference converts the coordinate out of int32 range, which is undefined; the engine writes 0.0f there.
+ * in: w x h floats, row pitch `pitch`; out: ow x oh floats, row pitch `opitch`; x0 + ow and y0 + oh must not exceed 2^31 - 1.
+ * VWB200_EARG, before the device is looked up, for a NULL params / in / out, a disparity kind without a disparity, an
+ * unknown enum, w, h, ow, oh (or dw, dh) <= 0, a pitch below its width, or an out that overlaps in or the disparity.
+ * ------------------------------------------------------------------------------------------- */
+enum { VWB200_WARP_HOMOGRAPHY = 0, VWB200_WARP_DISPARITY = 1 };
+enum { VWB200_INTERP_BILINEAR = 0, VWB200_INTERP_BICUBIC = 1, VWB200_INTERP_NEAREST = 2 };
+enum { VWB200_EDGE_ZERO = 0, VWB200_EDGE_CONSTANT = 1 };
+typedef struct { int32_t kind, interp, edge; double matrix[9]; } vwb200_warp_params;
+int vwb200_transform_image(const vwb200_warp_params* p, const float* in, int w, int h, ptrdiff_t pitch, const void* disparity, int dw,
+                           int dh, ptrdiff_t dpitch, int x0, int y0, float* out, int ow, int oh, ptrdiff_t opitch, int on_device,
+                           void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * vw::stereo::ParabolaSubpixelView::rasterize(dest, bbox) (src/vw/Stereo/ParabolaSubpixelView.h:27-117,
  * .cc:31-330): 3x3 AbsoluteCost patch around the integer disparity, 6x9 pseudo-inverse parabola fit,
  * offset kept when its norm is below 5.  disparity: cols x rows PixelMask<Vector2f> triples (same size as

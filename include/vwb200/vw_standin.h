@@ -12,6 +12,7 @@
 //   CropView<ImageT>            Image/Manipulation.h:82-146
 //   vw::rasterize               Image/ImageViewBase.h:283-316
 //   Exception hierarchy         Core/Exception.h:201-253
+//   Zero/ConstantEdgeExtension, Bilinear/Bicubic/NearestPixelInterpolation   tag types only (EdgeExtension.tcc, Interpolation.h)
 #pragma once
 #include <cstddef>
 #include <cstdint>
@@ -128,6 +129,13 @@ public:
 };
 template <class C> inline bool is_valid(PixelMask<C> const& p) { return p.valid() != 0; }
 static_assert(sizeof(PixelMask<Vector2f>) == 12, "PixelMask<Vector2f> must be 3 floats (Image/PixelMask.h:52-54)");
+
+// ---- edge extension and interpolation tags (Image/EdgeExtension.tcc:47-94, Image/Interpolation.h:113-225) -----------------
+struct ZeroEdgeExtension {};
+struct ConstantEdgeExtension {};
+struct BilinearInterpolation {};
+struct BicubicInterpolation {};
+struct NearestPixelInterpolation {};
 
 // ---- views -------------------------------------------------------------------------------------------
 template <class ImplT> struct ImageViewBase {                     // Image/ImageViewBase.h:57-64

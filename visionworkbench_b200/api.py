@@ -15,6 +15,8 @@ Names, argument order and error behaviour follow Vision Workbench:
   * disparity_subsample, disparity_upsample, get_disparity_range, disparity_range_mask, transform_disparities,
     transform_disparities_explicit (int32 or float32 disparities)
                               -- src/vw/Stereo/DisparityMap.h:48-66, 255-300, 1016-1057, 1190-1224, 1251-1358
+  * transform with HomographyTransform / DisparityTransform (float32 images; bilinear, bicubic, nearest; zero or
+    constant edges)           -- src/vw/Image/Transform.h:485-601, Math/Transform.h:369-389, Stereo/DisparityMap.h:1164-1187
 
 There is no CPU path: every call goes to libvwb200.so (hand-written sm_90a kernels) and raises if
 the library or a CUDA device is missing.  Inputs may be numpy arrays (staged through HBM by the
@@ -130,6 +132,7 @@ def lib():
         L.vwb200_get_disparity_range.argtypes = [I, P, I, I, Z, P, P, I, P]
         L.vwb200_disparity_range_mask.argtypes = [I, P, I, I, Z, P, P, P, Z, I, P]
         L.vwb200_transform_disparities.argtypes = [I, I, P, I, P, P, I, I, Z, P, Z, I, P]
+        L.vwb200_transform_image.argtypes = [C.POINTER(WarpParams), P, I, I, Z, P, I, I, Z, I, I, P, I, I, Z, I, P]
         L.vwb200_corr_create.argtypes = [C.POINTER(CorrParams), C.POINTER(P)]
         L.vwb200_corr_set_inputs.argtypes = [P, P, I, I, Z, P, I, I, Z, P, Z, P, Z, I]
         L.vwb200_corr_rasterize.argtypes = [P, I, I, I, I, P, Z, I, P]
@@ -563,6 +566,61 @@ def _transform(mode, matrix, do_round, box, disparity_map, out):
     _check(lib().vwb200_transform_disparities(_ptype(dt), mode, m.ctypes.data, int(bool(do_round)), sub, ptr, cols, rows, pitch, _ptr(o),
                                               pitch if out is not None else op, dev, _stream_ptr() if dev else None))
     return o
+
+
+# vwb200_transform_image's transform kinds, interpolations and edge extensions (include/vwb200.h)
+WARP_HOMOGRAPHY, WARP_DISPARITY = 0, 1
+INTERP_BILINEAR, INTERP_BICUBIC, INTERP_NEAREST = 0, 1, 2
+EDGE_ZERO, EDGE_CONSTANT = 0, 1
+
+
+class WarpParams(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("interp", C.c_int32), ("edge", C.c_int32), ("matrix", C.c_double * 9)]
+
+
+class HomographyTransform:
+    """vw::HomographyTransform(H) (Math/Transform.h:369-389): reverse() applies inverse(H), computed here with numpy (it agrees
+    with vw::math::inverse to rounding).  H must be 3 x 3 (ArgumentErr) and invertible (MathErr), as in the reference."""
+
+    def __init__(self, H):
+        self.H, self.H_inverse = _homography(H)
+
+
+class DisparityTransform:
+    """vw::stereo::DisparityTransform(disparity) (Stereo/DisparityMap.h:1164-1187) on a float32 (rows, cols, 3) {dx, dy, valid}
+    disparity, a numpy array or a CUDA tensor (the image it warps must be of the same kind): reverse(p) = p + (dx, dy) where
+    the pixel at p is valid, and (-1, p.y) elsewhere, outside the disparity included."""
+
+    def __init__(self, disparity):
+        if len(disparity.shape) != 3 or disparity.shape[2] != 3:
+            raise ArgumentErr("DisparityTransform: the disparity must be a float32 (rows, cols, 3) array or CUDA tensor")
+        self.disparity = disparity
+
+
+def transform(image, tx, bbox=None, edge=EDGE_ZERO, interp=INTERP_BILINEAR):
+    """vw::transform(image, tx[, bbox], edge, interp) (Image/Transform.h:485-601), rasterised: the float32 image (rows, cols),
+    numpy or CUDA, warped by a HomographyTransform or a DisparityTransform, over bbox (x0, y0, x1, y1) or a BBox2i of the
+    transformed image; None gives the image's own extent (0, 0, cols, rows).  The width / height form is
+    bbox=(0, 0, width, height).  Bit for bit the reference's where both reversed coordinates are finite with |c| < 2^30;
+    0.0 elsewhere.  Returns a new (y1 - y0, x1 - x0) float32 raster where the image lives."""
+    if not _is_torch(image) and _np(image, np.float32).ndim != 2:
+        raise ArgumentErr("transform: the image must be 2-D")
+    t, ptr, cols, rows, pitch, dev = _raster(image, np.float32)
+    x0, y0, x1, y1 = _bbox(bbox) if bbox is not None else (0, 0, cols, rows)
+    p = WarpParams(0, int(interp), int(edge))
+    keep, dptr, dw, dh, dpitch = None, None, 0, 0, 0
+    if isinstance(tx, HomographyTransform):
+        p.kind = WARP_HOMOGRAPHY
+        p.matrix[:] = [float(v) for v in np.asarray(tx.H_inverse, np.float64).reshape(9)]
+    elif isinstance(tx, DisparityTransform):
+        p.kind = WARP_DISPARITY
+        keep, dptr, dw, dh, dpitch, _ = _raster(tx.disparity, np.float32, channels=3, on_device=dev)
+    else:
+        raise ArgumentErr("transform: tx must be a HomographyTransform or a DisparityTransform")
+    out = _output(t, (max(y1 - y0, 0), max(x1 - x0, 0)), np.float32)
+    _check(lib().vwb200_transform_image(C.byref(p), ptr, cols, rows, pitch, dptr, dw, dh, dpitch, x0, y0, _ptr(out), x1 - x0, y1 - y0,
+                                        x1 - x0, dev, _stream_ptr() if dev else None))
+    return out
 
 
 def _disparity_arg(disparity):

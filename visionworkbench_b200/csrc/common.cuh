@@ -224,6 +224,11 @@ template <class T> int dispmap_range_mask_launch(const T* in, int w, int h, ptrd
 template <class T> int dispmap_transform_launch(int mode, const double* m9, int do_round, int sx0, int sy0, const T* in, int w, int h,
                                                 ptrdiff_t ip, T* out, ptrdiff_t op, cudaStream_t st);
 
+// ---- K8: transform(image, tx, edge, interp) of a float image over an output window (k8_warp.cu); pitches in elements ----------
+// disp (DispF, dw x dh, pitch dp) is read for VWB200_WARP_DISPARITY only
+int warp_launch(const vwb200_warp_params& p, const float* in, int w, int h, ptrdiff_t ip, const DispF* disp, int dw, int dh, ptrdiff_t dp,
+                int x0, int y0, float* out, int ow, int oh, ptrdiff_t op, cudaStream_t st);
+
 // ---- host-side restatement-free logic -----------------------------------------------------------
 struct Box { int x0, y0, x1, y1; };
 struct HostZone { Box img; Box disp; };

@@ -966,11 +966,12 @@ static int dispmap_check(const char* what, int pixel_type, const void* in, int w
   if (w < 0 || h < 0 || pitch < w) { set_error("%s: bad size %d x %d, pitch %td", what, w, h, pitch); return VWB200_EARG; }
   return VWB200_OK;
 }
-// [a0, a1) and [b0, b1): the bytes of an w x h / ow x oh raster of 12-byte pixels
-static bool rasters_overlap(const void* a, int w, int h, ptrdiff_t ap, const void* b, int ow, int oh, ptrdiff_t bp) {
+// [a0, a1) and [b0, b1): the bytes of an w x h / ow x oh raster of `apx` / `bpx`-byte pixels (disparity pixels by default)
+static bool rasters_overlap(const void* a, int w, int h, ptrdiff_t ap, const void* b, int ow, int oh, ptrdiff_t bp, size_t apx = 12,
+                            size_t bpx = 12) {
   if (w <= 0 || h <= 0 || ow <= 0 || oh <= 0) return false;
-  const uintptr_t a0 = (uintptr_t)a, a1 = a0 + ((size_t)(h - 1) * ap + w) * 12;
-  const uintptr_t b0 = (uintptr_t)b, b1 = b0 + ((size_t)(oh - 1) * bp + ow) * 12;
+  const uintptr_t a0 = (uintptr_t)a, a1 = a0 + ((size_t)(h - 1) * ap + w) * apx;
+  const uintptr_t b0 = (uintptr_t)b, b1 = b0 + ((size_t)(oh - 1) * bp + ow) * bpx;
   return a0 < b1 && b0 < a1;
 }
 // one resampling or per-pixel call: in (w x h) -> out (ow x oh), both staged through AbiCall.  launch(din, dp, dout, dop, st)
@@ -1631,6 +1632,45 @@ int vwb200_transform_disparities(int pixel_type, int mode, const double* matrix,
                      [&](auto* din, ptrdiff_t dp, auto* dout, ptrdiff_t dop, cudaStream_t st) {
                        return dispmap_transform_launch(mode, matrix, do_round != 0, sx0, sy0, din, w, h, dp, dout, dop, st);
                      });
+}
+
+// ---- K8: transform(image, tx, edge, interp) (Image/Transform.h:485-601) -----------------------------------------------------
+int vwb200_transform_image(const vwb200_warp_params* p, const float* in, int w, int h, ptrdiff_t pitch, const void* disparity, int dw,
+                           int dh, ptrdiff_t dpitch, int x0, int y0, float* out, int ow, int oh, ptrdiff_t opitch, int on_device,
+                           void* stream) {
+  if (!p || !in || !out) { set_error("transform_image: null params, input or output"); return VWB200_EARG; }
+  if (p->kind != VWB200_WARP_HOMOGRAPHY && p->kind != VWB200_WARP_DISPARITY) { set_error("transform_image: unknown transform kind %d", p->kind); return VWB200_EARG; }
+  if (p->interp != VWB200_INTERP_BILINEAR && p->interp != VWB200_INTERP_BICUBIC && p->interp != VWB200_INTERP_NEAREST) {
+    set_error("transform_image: unknown interpolation %d", p->interp);
+    return VWB200_EARG;
+  }
+  if (p->edge != VWB200_EDGE_ZERO && p->edge != VWB200_EDGE_CONSTANT) { set_error("transform_image: unknown edge extension %d", p->edge); return VWB200_EARG; }
+  if (w <= 0 || h <= 0 || pitch < w) { set_error("transform_image: bad image size %d x %d, pitch %td", w, h, pitch); return VWB200_EARG; }
+  if (ow <= 0 || oh <= 0 || opitch < ow) { set_error("transform_image: bad output size %d x %d, pitch %td", ow, oh, opitch); return VWB200_EARG; }
+  if ((long long)x0 + ow - 1 > INT_MAX || (long long)y0 + oh - 1 > INT_MAX) {
+    set_error("transform_image: the window (%d, %d, %d, %d) leaves the int32 pixel coordinates", x0, y0, ow, oh);
+    return VWB200_EARG;
+  }
+  const bool by_disp = p->kind == VWB200_WARP_DISPARITY;
+  if (by_disp && (!disparity || dw <= 0 || dh <= 0 || dpitch < dw)) {
+    set_error("transform_image: DisparityTransform needs a disparity (got %p, %d x %d, pitch %td)", disparity, dw, dh, dpitch);
+    return VWB200_EARG;
+  }
+  if (rasters_overlap(in, w, h, pitch, out, ow, oh, opitch, 4, 4) || (by_disp && rasters_overlap(disparity, dw, dh, dpitch, out, ow, oh, opitch, 12, 4))) {
+    set_error("transform_image: out overlaps the image or the disparity");
+    return VWB200_EARG;
+  }
+  VWB_TRY(ensure_device());
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
+  const float* din; ptrdiff_t dp;
+  VWB_TRY(c.in(in, w, h, pitch, on_device, &din, &dp));
+  const DispF* dd = nullptr; ptrdiff_t ddp = 0;
+  if (by_disp) VWB_TRY(c.in((const DispF*)disparity, dw, dh, dpitch, on_device, &dd, &ddp));
+  float* dout; ptrdiff_t dop;
+  VWB_TRY(c.out(out, ow, oh, opitch, on_device, &dout, &dop));
+  VWB_TRY(warp_launch(*p, din, w, h, dp, dd, dw, dh, ddp, x0, y0, dout, ow, oh, dop, c.st));
+  return c.finish();
 }
 
 // ---- the view -------------------------------------------------------------------------------------
