@@ -183,17 +183,32 @@ __global__ void pack_right_kernel(ImgF img, float vmin, FastGeom g, uint16_t* __
 }
 
 // ---- one pass: 8 consecutive dx (octet g) x 8 columns per lane, sliding down the warp's rows ----------------
-__device__ __forceinline__ void unpack8(const uint4 v, int (&o)[8]) {
-  o[0] = v.x & 0xffff; o[1] = v.x >> 16; o[2] = v.y & 0xffff; o[3] = v.y >> 16;
-  o[4] = v.z & 0xffff; o[5] = v.z >> 16; o[6] = v.w & 0xffff; o[7] = v.w >> 16;
+// The AbsoluteCost row step is bound by the integer ALU pipe (VABSDIFF, IADD3, VIADDMNMX), so it splits the halves on
+// the FMA pipe: hi = IMAD.HI(v, 2^16), lo = IMAD(hi, -2^16, v).  Written as `v >> 16` / `v & 0xffff`, ptxas emits SHF /
+// LOP3 on the ALU pipe, which the SquaredCost step keeps: its (a-b)^2 already loads the FMA pipe more than the ALU pipe.
+template <bool FMA>
+__device__ __forceinline__ void unpack2(const uint32_t v, int& lo, int& hi) {
+  if (FMA) {
+    uint32_t h, l;
+    asm("mul.hi.u32 %0, %1, 65536;" : "=r"(h) : "r"(v));
+    asm("mad.lo.u32 %0, %1, -65536, %2;" : "=r"(l) : "r"(h), "r"(v));
+    lo = (int)l; hi = (int)h;
+  } else {
+    lo = v & 0xffff; hi = v >> 16;
+  }
 }
+template <bool FMA>
+__device__ __forceinline__ void unpack8(const uint4 v, int (&o)[8]) {
+  unpack2<FMA>(v.x, o[0], o[1]); unpack2<FMA>(v.y, o[2], o[3]); unpack2<FMA>(v.z, o[4], o[5]); unpack2<FMA>(v.w, o[6], o[7]);
+}
+template <bool FMA>
 __device__ __forceinline__ void load_row(const uint16_t* lrow, const uint16_t* rrow, int (&Lv)[8], int (&Rv)[16]) {
-  unpack8(*reinterpret_cast<const uint4*>(lrow), Lv);
+  unpack8<FMA>(*reinterpret_cast<const uint4*>(lrow), Lv);
   int t[8];
-  unpack8(*reinterpret_cast<const uint4*>(rrow), t);
+  unpack8<FMA>(*reinterpret_cast<const uint4*>(rrow), t);
 #pragma unroll
   for (int i = 0; i < 8; ++i) Rv[i] = t[i];
-  unpack8(*reinterpret_cast<const uint4*>(rrow + 8), t);
+  unpack8<FMA>(*reinterpret_cast<const uint4*>(rrow + 8), t);
 #pragma unroll
   for (int i = 0; i < 8; ++i) Rv[8 + i] = t[i];
 }
@@ -212,9 +227,15 @@ __device__ __forceinline__ void fast_pass(const uint16_t* __restrict__ ltile, co
                                           uint32_t* __restrict__ best, unsigned long long* __restrict__ keys,
                                           int lane, int g, int ky, int ring_slots, int rw, int ring_base, int idx_base, int nrows, int nb) {
   int V[8][F_B];
-  const uint16_t* lp = ltile + 8 * lane;                       // + row*256            (16-byte aligned)
-  const uint16_t* rp = rring + 8 * (lane + g);                 // + slot*rw            (16-byte aligned)
-  int slot_new = ring_base;                                     // ring slot of right row (dy + t)
+  // Row pointers: the left rows advance by 256, the right rows by rw and wrap around the ring with one compare and
+  // subtract, so a row step computes no slot * rw.
+  const uint16_t* lnew = ltile + 8 * lane;                      // left row y + ky - 1  (16-byte aligned)
+  const uint16_t* lold = lnew;                                  // left row y - 1
+  const uint16_t* const rring_lane = rring + 8 * (lane + g);
+  const uint16_t* const rend = rring_lane + ring_slots * rw;
+  const int rspan = ring_slots * rw;
+  const uint16_t* rnew = rring_lane + ring_base * rw;           // right row dy + y + ky - 1
+  const uint16_t* rold = rnew;                                  // right row dy + y - 1
   // ---- seed: first ky rows ----
 #pragma unroll
   for (int a = 0; a < 8; ++a)
@@ -222,35 +243,18 @@ __device__ __forceinline__ void fast_pass(const uint16_t* __restrict__ ltile, co
     for (int b = 0; b < F_B; ++b) V[a][b] = 0;
   for (int t = 0; t < ky; ++t) {
     int Lv[8], Rv[16];
-    load_row(lp + t * F_COLS, rp + slot_new * rw, Lv, Rv);
+    load_row<true>(lnew, rnew, Lv, Rv);
 #pragma unroll
     for (int a = 0; a < 8; ++a)
 #pragma unroll
       for (int b = 0; b < F_B; ++b) V[a][b] = __sad(Lv[a], Rv[a + b], V[a][b]);
-    if (++slot_new == ring_slots) slot_new = 0;
+    lnew += F_COLS;
+    rnew += rw; if (rnew == rend) rnew -= rspan;
   }
-  int slot_old = ring_base;
-  for (int y = 0; y < nrows; ++y) {
-    if (y > 0) {
-      {
-        int Lv[8], Rv[16];
-        load_row(lp + (y + ky - 1) * F_COLS, rp + slot_new * rw, Lv, Rv);
-#pragma unroll
-        for (int a = 0; a < 8; ++a)
-#pragma unroll
-          for (int b = 0; b < F_B; ++b) V[a][b] = __sad(Lv[a], Rv[a + b], V[a][b]);
-      }
-      {
-        int Lo[8], Ro[16];
-        load_row(lp + (y - 1) * F_COLS, rp + slot_old * rw, Lo, Ro);
-#pragma unroll
-        for (int a = 0; a < 8; ++a)
-#pragma unroll
-          for (int b = 0; b < F_B; ++b) V[a][b] -= __sad(Lo[a], Ro[a + b], 0);
-      }
-      if (++slot_new == ring_slots) slot_new = 0;
-      if (++slot_old == ring_slots) slot_old = 0;
-    }
+  uint32_t* brow = best + lane;
+  // row y = 0 has no sliding update; the loop leaves after the arg-best of its last row, so the update of every
+  // following row needs no test of y
+  for (int y = 0;;) {
     // ---- horizontal window sums + min over the 8 dx (keys = cost*8 + b) ----
     int m[8];
 #pragma unroll
@@ -266,17 +270,40 @@ __device__ __forceinline__ void fast_pass(const uint16_t* __restrict__ ltile, co
     }
     // ---- running best: high words hold cost*8 | 7, so m <= s <=> cost <= best cost.  Equal costs are candidates
     //      too: another warp may hold the same cost at a later disparity ----
-    uint32_t* brow = best + y * F_COLS + lane;
-    unsigned long long* krow = keys + y * F_COLS + lane;
-    uint32_t s8[8];
     bool cand = false;
 #pragma unroll
-    for (int r = 0; r < 8; ++r) { s8[r] = brow[r * 32]; cand |= ((uint32_t)m[r] <= s8[r]); }
+    for (int r = 0; r < 8; ++r) cand |= ((uint32_t)m[r] <= brow[r * 32]);
     if (cand) {                // rare once the search has seen the neighbourhood of the true match
+      // The thresholds are read again (volatile), so the common path keeps one predicate rather than eight.  A threshold
+      // lowered meanwhile by another warp only holds back an offer that could not win.
+      const volatile uint32_t* vrow = brow;
+      unsigned long long* krow = keys + y * F_COLS + lane;
 #pragma unroll
       for (int r = 0; r < 8; ++r)
-        if ((uint32_t)m[r] <= s8[r]) offer_key(brow + r * 32, krow + r * 32, (uint32_t)m[r] | 7u, (uint32_t)(idx_base + (m[r] & 7)));
+        if ((uint32_t)m[r] <= vrow[r * 32]) offer_key(brow + r * 32, krow + r * 32, (uint32_t)m[r] | 7u, (uint32_t)(idx_base + (m[r] & 7)));
     }
+    if (++y == nrows) break;
+    brow += F_COLS;
+    // ---- slide the vertical sums down one row: + row y + ky - 1, - row y - 1 ----
+    {
+      int Lv[8], Rv[16];
+      load_row<true>(lnew, rnew, Lv, Rv);
+#pragma unroll
+      for (int a = 0; a < 8; ++a)
+#pragma unroll
+        for (int b = 0; b < F_B; ++b) V[a][b] = __sad(Lv[a], Rv[a + b], V[a][b]);
+    }
+    {
+      int Lo[8], Ro[16];
+      load_row<true>(lold, rold, Lo, Ro);
+#pragma unroll
+      for (int a = 0; a < 8; ++a)
+#pragma unroll
+        for (int b = 0; b < F_B; ++b) V[a][b] -= __sad(Lo[a], Ro[a + b], 0);
+    }
+    lnew += F_COLS; lold += F_COLS;
+    rnew += rw; if (rnew == rend) rnew -= rspan;
+    rold += rw; if (rold == rend) rold -= rspan;
   }
 }
 
@@ -298,7 +325,7 @@ __device__ __forceinline__ void fast_pass_sq(const uint16_t* __restrict__ ltile,
   int slot_new = ring_base;
   for (int t = 0; t < ky; ++t) {
     int Lv[8], Rv[16];
-    load_row(lp + t * F_COLS, rp + slot_new * rw, Lv, Rv);
+    load_row<false>(lp + t * F_COLS, rp + slot_new * rw, Lv, Rv);
 #pragma unroll
     for (int a = 0; a < 8; ++a)
 #pragma unroll
@@ -310,7 +337,7 @@ __device__ __forceinline__ void fast_pass_sq(const uint16_t* __restrict__ ltile,
     if (y > 0) {
       {
         int Lv[8], Rv[16];
-        load_row(lp + (y + ky - 1) * F_COLS, rp + slot_new * rw, Lv, Rv);
+        load_row<false>(lp + (y + ky - 1) * F_COLS, rp + slot_new * rw, Lv, Rv);
 #pragma unroll
         for (int a = 0; a < 8; ++a)
 #pragma unroll
@@ -318,7 +345,7 @@ __device__ __forceinline__ void fast_pass_sq(const uint16_t* __restrict__ ltile,
       }
       {
         int Lo[8], Ro[16];
-        load_row(lp + (y - 1) * F_COLS, rp + slot_old * rw, Lo, Ro);
+        load_row<false>(lp + (y - 1) * F_COLS, rp + slot_old * rw, Lo, Ro);
 #pragma unroll
         for (int a = 0; a < 8; ++a)
 #pragma unroll
