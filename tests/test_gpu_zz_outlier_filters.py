@@ -206,9 +206,9 @@ def largest_half_h(hy, words):
 @pytest.mark.parametrize("dtype", TYPES, ids=["i32", "f32"])
 @pytest.mark.parametrize("method", METHODS)
 def test_window_limits(vwb, ou, method, dtype):
-    """the largest accepted window, and VWB200_ENOIMPL one step above it.  The integer thresh filters run the level loop's
-    kernel (two words per staged pixel); the others stage three."""
-    words = 2 if (method == R.THRESH and dtype == np.int32) else 3
+    """the largest accepted window, and VWB200_ENOIMPL one step above it.  The thresh filters stage two words per pixel
+    (validity folded into dx); mean and stddev stage three."""
+    words = 2 if method == R.THRESH else 3
     d = R.random_disparity(3, (12, 40), 0.3, dtype)
     for hy in (1, 20):
         hx = largest_half_h(hy, words)
@@ -247,8 +247,8 @@ for dt, tn in ((np.int32, "vwb200_dispi"), (np.float32, "DispF")):
 
 
 def test_kernel_trace():
-    """each filter ran its kernel: integer thresh the level loop's rm_outliers_kernel, the others
-    outlier_pass1_kernel<pixel type, method>; the cleanup composites add cleanup_pass2_kernel<pixel type>"""
+    """each filter ran its kernel, outlier_pass1_kernel<pixel type, method> and no other pass-1 kernel; the cleanup
+    composites add cleanup_pass2_kernel<pixel type>"""
     here = os.path.dirname(os.path.abspath(__file__))
     env = dict(os.environ, PYTHONPATH=os.pathsep.join([os.path.dirname(here), here]), PYTHONNOUSERSITE="1")
     r = subprocess.run([sys.executable, "-c", TRACE_SCRIPT], cwd=here, env=env, capture_output=True, text=True, timeout=600)
@@ -257,10 +257,7 @@ def test_kernel_trace():
     assert len(cases) == 12, r.stdout
     for tn, m, cleanup, names in cases:
         names = names.split("|")
-        if tn == "vwb200_dispi" and m == "0":
-            want = re.compile(r"\brm_outliers_kernel\(")
-        else:
-            want = re.compile(rf"outlier_pass1_kernel<(vwb200::)?{tn}, (\(int\))?{m}>")
+        want = re.compile(rf"outlier_pass1_kernel<(vwb200::)?{tn}, (\(int\))?{m}>")
         assert any(want.search(n) for n in names), (tn, m, cleanup, names)
-        assert any("outlier_pass1_kernel" in n for n in names) != (tn == "vwb200_dispi" and m == "0"), names
+        assert all(want.search(n) or "cleanup_pass2_kernel" in n for n in names), names
         assert any("cleanup_pass2_kernel" in n for n in names) == (cleanup == "1"), names

@@ -179,9 +179,6 @@ int sgm_finalize_launch(const float* sub, const vwb200_dispi* disp, int w, int a
                         int ow, int oh, cudaStream_t st);
 // disparity_blob_filter; work: 2 * w * h ints
 int blob_filter_launch(vwb200_dispi* d, int w, int h, int area, int* work, cudaStream_t st);
-// pass 1 of the outlier filter evaluated over [x0,x0+ow) x [y0,y0+oh) of the constant-edge-extended input
-int rm_outliers_launch(const vwb200_dispi* in, int w, int h, int hx, int hy, double pt, double rt,
-                       int x0, int y0, int ow, int oh, vwb200_dispi* out, cudaStream_t st);
 // pass 2 (1,1,3.0,0.20) reading the padded pass-1 buffer (w+2)x(h+2)
 int cleanup_pass2_launch(const vwb200_dispi* p1, int w, int h, vwb200_dispi* out, cudaStream_t st);
 int cleanup_pass2_launch(const DispF* p1, int w, int h, DispF* out, cudaStream_t st);

@@ -444,21 +444,31 @@ static int filtered_region(ImgF img, int mode, float width, Box reg, float** out
   return log_region_launch(g, ew, big.x0, big.y0, img.w, img.h, reg.x0, reg.y0, w, h, o, st);
 }
 
-// The outlier filter chain (CorrelationView.cc:713-744): pass 1 of rm_outliers_using_thresh, either unpadded or padded and
-// followed by pass 2 (disparity_cleanup_using_thresh), then disparity_mask when masks are given.  in -> out, w x h, dense;
-// out may be in when there are masks.
+// ---- the outlier filters on either pixel type (Stereo/DisparityMap.h:318-767) ------------------------------------
+// in: device raster of w x h pixels, row pitch ip; out: dense w x h.  Pass 1 of the method, unpadded, or padded and followed
+// by pass 2 (the disparity_cleanup_using_* composites).
+template <class T>
+static int outlier_filter_run(const vwb200_outlier_params& p, const T* in, int w, int h, ptrdiff_t ip, T* out, Arena& ar, cudaStream_t st) {
+  if (!p.cleanup)
+    return outlier_pass1_launch(p.method, in, w, h, ip, p.half_h, p.half_v, p.pixel_threshold, p.rejection_threshold, p.max_mean_diff,
+                                0, 0, w, h, out, (ptrdiff_t)w, st);
+  T* t1;
+  VWB_TRY(ar.alloc(&t1, (size_t)(w + 2) * (h + 2)));
+  VWB_TRY(outlier_pass1_launch(p.method, in, w, h, ip, p.half_h, p.half_v, p.pixel_threshold, p.rejection_threshold, p.max_mean_diff,
+                               -1, -1, w + 2, h + 2, t1, (ptrdiff_t)w + 2, st));
+  return cleanup_pass2_launch(t1, w, h, out, st);
+}
+
+// The level loop's outlier filter chain (CorrelationView.cc:713-744): rm_outliers_using_thresh, or
+// disparity_cleanup_using_thresh, then disparity_mask when masks are given.  in -> out, w x h, dense; out may be in when
+// there are masks.
 static int outlier_filter_chain(const vwb200_dispi* in, int w, int h, int hx, int hy, double pt, double rt, bool cleanup, ImgB lmask,
                                 ImgB rmask, vwb200_dispi* out, Arena& ar, cudaStream_t st) {
-  vwb200_dispi *t1, *t2 = out;
-  if (lmask.p) VWB_TRY(ar.alloc(&t2, (size_t)w * h));
-  if (cleanup) {
-    VWB_TRY(ar.alloc(&t1, (size_t)(w + 2) * (h + 2)));
-    VWB_TRY(rm_outliers_launch(in, w, h, hx, hy, pt, rt, -1, -1, w + 2, h + 2, t1, st));
-    VWB_TRY(cleanup_pass2_launch(t1, w, h, t2, st));
-  } else {
-    VWB_TRY(rm_outliers_launch(in, w, h, hx, hy, pt, rt, 0, 0, w, h, t2, st));
-  }
-  if (lmask.p) VWB_TRY(disparity_mask_launch(t2, w, h, lmask, rmask, out, st));
+  vwb200_dispi* t = out;
+  if (lmask.p) VWB_TRY(ar.alloc(&t, (size_t)w * h));
+  const vwb200_outlier_params p{VWB200_OUTLIERS_THRESH, cleanup, hx, hy, pt, rt, 0.0};
+  VWB_TRY(outlier_filter_run(p, in, w, h, (ptrdiff_t)w, t, ar, st));
+  if (lmask.p) VWB_TRY(disparity_mask_launch(t, w, h, lmask, rmask, out, st));
   return VWB200_OK;
 }
 
@@ -918,33 +928,7 @@ struct AbiCall {
   }
 };
 
-// ---- the outlier filters on either pixel type (Stereo/DisparityMap.h:318-767) ------------------------------------
-// in: device raster of w x h pixels, row pitch ip; out: dense w x h.  Integer thresh runs the level loop's chain itself;
-// the other five filters run pass 1 of their method, unpadded, or padded and followed by pass 2 as in outlier_filter_chain.
-template <class T>
-static int outlier_filter_run(const vwb200_outlier_params& p, const T* in, int w, int h, ptrdiff_t ip, T* out, Arena& ar, cudaStream_t st) {
-  if constexpr (std::is_same<T, vwb200_dispi>::value) {
-    if (p.method == VWB200_OUTLIERS_THRESH) {
-      if (ip != w) {                                     // the thresh kernel reads a dense raster
-        vwb200_dispi* d;
-        VWB_TRY(ar.alloc(&d, (size_t)w * h));
-        VWB_CUDA(cudaMemcpy2DAsync(d, (size_t)w * sizeof(T), in, (size_t)ip * sizeof(T), (size_t)w * sizeof(T), h, cudaMemcpyDeviceToDevice, st));
-        in = d;
-      }
-      return outlier_filter_chain(in, w, h, p.half_h, p.half_v, p.pixel_threshold, p.rejection_threshold, p.cleanup != 0, ImgB{}, ImgB{},
-                                  out, ar, st);
-    }
-  }
-  if (!p.cleanup)
-    return outlier_pass1_launch(p.method, in, w, h, ip, p.half_h, p.half_v, p.pixel_threshold, p.rejection_threshold, p.max_mean_diff,
-                                0, 0, w, h, out, (ptrdiff_t)w, st);
-  T* t1;
-  VWB_TRY(ar.alloc(&t1, (size_t)(w + 2) * (h + 2)));
-  VWB_TRY(outlier_pass1_launch(p.method, in, w, h, ip, p.half_h, p.half_v, p.pixel_threshold, p.rejection_threshold, p.max_mean_diff,
-                               -1, -1, w + 2, h + 2, t1, (ptrdiff_t)w + 2, st));
-  return cleanup_pass2_launch(t1, w, h, out, st);
-}
-// one vwb200_outlier_filter call: the input staged or used in place, the output written densely and copied back
+// one outlier filter call: the input staged or used in place, the output written densely and copied back
 template <class T>
 static int outlier_filter_typed(const vwb200_outlier_params& p, const T* in, int w, int h, ptrdiff_t pitch, T* out, ptrdiff_t opitch,
                                 int on_device, void* stream) {
@@ -1487,35 +1471,33 @@ int vwb200_cross_corr_consistency_check(vwb200_dispi* l2r, int lw, int lh, ptrdi
   return c.finish();
 }
 
-// the outlier filters and the mask on dense w x h rasters
-static int filter_common(int which, const vwb200_dispi* in, int w, int h, int hx, int hy, double pt, double rt,
-                         const uint8_t* lm, const uint8_t* rm, int rmw, int rmh, vwb200_dispi* out, int on_device, void* stream) {
+// the integer thresh filters on dense w x h rasters
+static int thresh_filter(bool cleanup, const vwb200_dispi* in, int w, int h, int hx, int hy, double pt, double rt, vwb200_dispi* out,
+                         int on_device, void* stream) {
+  if (!in || !out || w <= 0 || h <= 0) { set_error("disparity filter: bad arguments"); return VWB200_EARG; }
+  VWB_TRY(ensure_device());
+  const vwb200_outlier_params p{VWB200_OUTLIERS_THRESH, cleanup, hx, hy, pt, rt, 0.0};
+  return outlier_filter_typed(p, in, w, h, (ptrdiff_t)w, out, (ptrdiff_t)w, on_device, stream);
+}
+int vwb200_rm_outliers_using_thresh(const vwb200_dispi* in, int w, int h, int hx, int hy, double pt, double rt, vwb200_dispi* out, int on_device, void* stream) {
+  return thresh_filter(false, in, w, h, hx, hy, pt, rt, out, on_device, stream);
+}
+int vwb200_disparity_cleanup_using_thresh(const vwb200_dispi* in, int w, int h, int hx, int hy, double pt, double rt, vwb200_dispi* out, int on_device, void* stream) {
+  return thresh_filter(true, in, w, h, hx, hy, pt, rt, out, on_device, stream);
+}
+int vwb200_disparity_mask(const vwb200_dispi* in, int w, int h, const uint8_t* lm, const uint8_t* rm, int rmw, int rmh, vwb200_dispi* out, int on_device, void* stream) {
+  if (!lm || !rm) { set_error("disparity_mask: null mask"); return VWB200_EARG; }
   if (!in || !out || w <= 0 || h <= 0) { set_error("disparity filter: bad arguments"); return VWB200_EARG; }
   VWB_TRY(ensure_device());
   AbiCall c;
   VWB_TRY(c.open(stream, on_device));
-  const vwb200_dispi* din; vwb200_dispi* dout; ptrdiff_t dp;
+  const vwb200_dispi* din; vwb200_dispi* dout; const uint8_t *dlm, *drm; ptrdiff_t dp, p1, p2;
   VWB_TRY(c.in(in, w, h, (ptrdiff_t)w, on_device, &din, &dp));
   VWB_TRY(c.out(out, w, h, (ptrdiff_t)w, on_device, &dout, &dp));
-  if (which < 2) {
-    VWB_TRY(outlier_filter_chain(din, w, h, hx, hy, pt, rt, which == 1, ImgB{}, ImgB{}, dout, c.ar, c.st));
-  } else {
-    const uint8_t *dlm, *drm; ptrdiff_t p1, p2;
-    VWB_TRY(c.in(lm, w, h, (ptrdiff_t)w, on_device, &dlm, &p1));
-    VWB_TRY(c.in(rm, rmw, rmh, (ptrdiff_t)rmw, on_device, &drm, &p2));
-    VWB_TRY(disparity_mask_launch(din, w, h, ImgB{dlm, w, h, p1}, ImgB{drm, rmw, rmh, p2}, dout, c.st));
-  }
+  VWB_TRY(c.in(lm, w, h, (ptrdiff_t)w, on_device, &dlm, &p1));
+  VWB_TRY(c.in(rm, rmw, rmh, (ptrdiff_t)rmw, on_device, &drm, &p2));
+  VWB_TRY(disparity_mask_launch(din, w, h, ImgB{dlm, w, h, p1}, ImgB{drm, rmw, rmh, p2}, dout, c.st));
   return c.finish();
-}
-int vwb200_rm_outliers_using_thresh(const vwb200_dispi* in, int w, int h, int hx, int hy, double pt, double rt, vwb200_dispi* out, int on_device, void* stream) {
-  return filter_common(0, in, w, h, hx, hy, pt, rt, nullptr, nullptr, 0, 0, out, on_device, stream);
-}
-int vwb200_disparity_cleanup_using_thresh(const vwb200_dispi* in, int w, int h, int hx, int hy, double pt, double rt, vwb200_dispi* out, int on_device, void* stream) {
-  return filter_common(1, in, w, h, hx, hy, pt, rt, nullptr, nullptr, 0, 0, out, on_device, stream);
-}
-int vwb200_disparity_mask(const vwb200_dispi* in, int w, int h, const uint8_t* lm, const uint8_t* rm, int rmw, int rmh, vwb200_dispi* out, int on_device, void* stream) {
-  if (!lm || !rm) { set_error("disparity_mask: null mask"); return VWB200_EARG; }
-  return filter_common(2, in, w, h, 1, 1, 0, 0, lm, rm, rmw, rmh, out, on_device, stream);
 }
 
 int vwb200_outlier_filter(const vwb200_outlier_params* p, int pixel_type, const void* in, int w, int h, ptrdiff_t pitch, void* out,
@@ -1530,11 +1512,9 @@ int vwb200_outlier_filter(const vwb200_outlier_params* p, int pixel_type, const 
     return VWB200_EARG;
   }
   if (w < 0 || h < 0 || pitch < w || opitch < w) { set_error("outlier_filter: bad size %d x %d, pitches %td, %td", w, h, pitch, opitch); return VWB200_EARG; }
-  if (w > 0 && h > 0) {                                  // each output pixel reads a window of the input: no overlap
-    const size_t px = 12;
-    const uintptr_t a0 = (uintptr_t)in, a1 = a0 + ((size_t)(h - 1) * pitch + w) * px;
-    const uintptr_t b0 = (uintptr_t)out, b1 = b0 + ((size_t)(h - 1) * opitch + w) * px;
-    if (a0 < b1 && b0 < a1) { set_error("outlier_filter: out overlaps in (the filters are not in place)"); return VWB200_EARG; }
+  if (rasters_overlap(in, w, h, pitch, out, w, h, opitch)) {   // each output pixel reads a window of the input
+    set_error("outlier_filter: out overlaps in (the filters are not in place)");
+    return VWB200_EARG;
   }
   VWB_TRY(ensure_device());
   if (!w || !h) return VWB200_OK;

@@ -75,67 +75,17 @@ int zone_post_launch(const Tile* d_tiles, int ntiles, const Zone* d_zones, const
   return VWB200_OK;
 }
 
-// ---- K4: RmOutliersUsingThreshFunc (DisparityMap.h:359-386) -----------------------------------------
-// Evaluated at (cx,cy) of the ConstantEdgeExtension of `in`; the output window may extend past the
-// image (second-pass quirk of disparity_cleanup_using_thresh, Image/PerPixelAccessorViews.h:63-85).
-// CTA stages its (tile + halo) neighbourhood in shared memory (dx,dy packed, validity folded in).
-static constexpr int RO_TW = 32, RO_TH = 8;
-__global__ void __launch_bounds__(RO_TW * RO_TH)
-rm_outliers_kernel(const vwb200_dispi* __restrict__ in, int w, int h, int hx, int hy, double pt, double rt,
-                   int x0, int y0, int ow, int oh, vwb200_dispi* __restrict__ out) {
-  extern __shared__ int sm[];                // [sh][sw] x {dx, dy}; invalid -> dx = INT_MIN
-  const int sw = RO_TW + 2 * hx, sh = RO_TH + 2 * hy;
-  int* sdx = sm; int* sdy = sm + sw * sh;
-  const int bx = x0 + blockIdx.x * RO_TW, by = y0 + blockIdx.y * RO_TH;
-  const int tid = threadIdx.y * RO_TW + threadIdx.x;
-  for (int k = tid; k < sw * sh; k += RO_TW * RO_TH) {
-    const int sx = k % sw, sy = k / sw;
-    const vwb200_dispi v = in[(ptrdiff_t)clampi3(by - hy + sy, 0, h - 1) * w + clampi3(bx - hx + sx, 0, w - 1)];
-    sdx[k] = v.valid ? v.dx : INT_MIN;
-    sdy[k] = v.dy;
-  }
-  __syncthreads();
-  const int ox = blockIdx.x * RO_TW + threadIdx.x, oy = blockIdx.y * RO_TH + threadIdx.y;
-  if (ox >= ow || oy >= oh) return;
-  const int cx = threadIdx.x + hx, cy = threadIdx.y + hy;
-  // the centre pixel keeps its child values even when invalid ("return *acc")
-  vwb200_dispi c = in[(ptrdiff_t)clampi3(y0 + oy, 0, h - 1) * w + clampi3(x0 + ox, 0, w - 1)];
-  if (c.valid) {
-    int matched = 0;
-    const int total = (2 * hx + 1) * (2 * hy + 1);
-    for (int yk = -hy; yk <= hy; ++yk) {
-      const int* rdx = sdx + (cy + yk) * sw + cx;
-      const int* rdy = sdy + (cy + yk) * sw + cx;
-      for (int xk = -hx; xk <= hx; ++xk) {
-        const int ndx = rdx[xk];
-        if (ndx != INT_MIN && fabs((double)(c.dx - ndx)) <= pt && fabs((double)(c.dy - rdy[xk])) <= pt) ++matched;
-      }
-    }
-    if (((double)matched / (double)total) < rt) { c.dx = 0; c.dy = 0; c.valid = 0; }
-  }
-  out[(ptrdiff_t)oy * ow + ox] = c;
-}
-int rm_outliers_launch(const vwb200_dispi* in, int w, int h, int hx, int hy, double pt, double rt,
-                       int x0, int y0, int ow, int oh, vwb200_dispi* out, cudaStream_t st) {
-  if (ow <= 0 || oh <= 0) return VWB200_OK;
-  if (hx <= 0 || hy <= 0) { set_error("RmOutliersFunc: half kernel sizes must be non-zero."); return VWB200_EARG; }  // DisparityMap.h:345-346
-  const size_t smem = (size_t)(RO_TW + 2 * hx) * (RO_TH + 2 * hy) * 2 * sizeof(int);
-  if (smem > 200 * 1024) { set_error("outlier filter half kernel %dx%d too large", hx, hy); return VWB200_ENOIMPL; }
-  VWB_CUDA(cudaFuncSetAttribute(rm_outliers_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));   // per-function state shared by all host threads: device maximum
-  dim3 b(RO_TW, RO_TH), g((ow + RO_TW - 1) / RO_TW, (oh + RO_TH - 1) / RO_TH);
-  rm_outliers_kernel<<<g, b, smem, st>>>(in, w, h, hx, hy, pt, rt, x0, y0, ow, oh, out);
-  VWB_LAUNCH_CHECK();
-  return VWB200_OK;
-}
-
 // The pixel types of the outlier filters: PixelMask<Vector2i> and PixelMask<Vector2f>, valid when valid != 0.  absdiff is
 // the reference's fabs((*acc)[0] - (*col_acc)[0]): the difference in the pixel type (int, or a rounded float), then a
 // double.  key is |dx| + |dy| in the pixel type (RmOutliersUsingMeanFunc's len, DisparityMap.h:504) as an order-preserving
-// uint32: the int itself, or the float's fkey (the sum is never negative); kval is the key's value as a double.
+// uint32: the int itself, or the float's fkey (the sum is never negative); kval is the key's value as a double.  The thresh
+// filter stages an invalid pixel's dx as `absent` (INT_MIN, or NaN), which `present` tells apart.
 template <class T> struct OutlierPx;
 template <> struct OutlierPx<vwb200_dispi> {
   typedef int V;
   static __device__ __forceinline__ bool valid(const vwb200_dispi& p) { return p.valid != 0; }
+  static __device__ __forceinline__ int absent() { return INT_MIN; }
+  static __device__ __forceinline__ bool present(int dx) { return dx != INT_MIN; }
   static __device__ __forceinline__ double absdiff(int a, int b) { return fabs((double)(a - b)); }
   static __device__ __forceinline__ unsigned key(int dx, int dy) { return (unsigned)(abs(dx) + abs(dy)); }
   static __device__ __forceinline__ double kval(unsigned k) { return (double)(int)k; }
@@ -143,6 +93,8 @@ template <> struct OutlierPx<vwb200_dispi> {
 template <> struct OutlierPx<DispF> {
   typedef float V;
   static __device__ __forceinline__ bool valid(const DispF& p) { return p.valid != 0.0f; }
+  static __device__ __forceinline__ float absent() { return __int_as_float(0x7fffffff); }
+  static __device__ __forceinline__ bool present(float dx) { return !isnan(dx); }
   static __device__ __forceinline__ double absdiff(float a, float b) { return (double)fabsf(__fsub_rn(a, b)); }
   static __device__ __forceinline__ unsigned key(float dx, float dy) { return fkey(__fadd_rn(fabsf(dx), fabsf(dy))); }
   static __device__ __forceinline__ double kval(unsigned k) { return (double)kfloat(k); }
@@ -186,9 +138,12 @@ int cleanup_pass2_launch(const DispF* p1, int w, int h, DispF* out, cudaStream_t
 
 // ---- K4 on both pixel types: pass 1 of rm_outliers_using_thresh / _mean / _stddev ----------------------------------------
 // (DisparityMap.h:359-386, :484-553, :646-723).  One thread per output pixel over [x0,x0+ow) x [y0,y0+oh) of the
-// ConstantEdgeExtension of `in`, as rm_outliers_kernel does; the CTA stages its tile + halo in shared memory as {dx}, {dy}
-// and a key word: kNoKeyO for an invalid pixel, else |dx| + |dy| as a key (mean) or 0.  Every sum runs in the reference's
-// row-major order with explicitly rounded operations (no contraction).
+// ConstantEdgeExtension of `in`; the output window may extend past the image (the padded first pass of the cleanup
+// composites, Image/PerPixelAccessorViews.h:63-85).  The CTA stages its tile + halo in shared memory as {dx}, {dy}, and for
+// mean and stddev a key word: kNoKeyO for an invalid pixel, else |dx| + |dy| as a key (mean) or 0.  Thresh folds validity
+// into dx instead (Px::absent), so its hot loop reads two planes.  Every sum runs in the reference's row-major order with
+// explicitly rounded operations (no contraction).
+static constexpr int RO_TW = 32, RO_TH = 8;
 static constexpr unsigned kNoKeyO = 0xFFFFFFFFu;   // above every key of a finite |dx| + |dy|
 static constexpr size_t kOutlierSmemMax = 200 * 1024;
 
@@ -202,14 +157,14 @@ outlier_pass1_kernel(const T* __restrict__ in, int w, int h, ptrdiff_t ipitch, i
   const int sw = RO_TW + 2 * hx, sh = RO_TH + 2 * hy, sn = sw * sh;
   V* sdx = reinterpret_cast<V*>(osm);
   V* sdy = sdx + sn;
-  unsigned* skey = osm + 2 * sn;
+  unsigned* skey = osm + 2 * sn;                          // mean and stddev only
   const int bx = x0 + blockIdx.x * RO_TW, by = y0 + blockIdx.y * RO_TH;
   for (int k = threadIdx.y * RO_TW + threadIdx.x; k < sn; k += RO_TW * RO_TH) {
     const int sx = k % sw, sy = k / sw;
     const T v = in[(ptrdiff_t)clampi3(by - hy + sy, 0, h - 1) * ipitch + clampi3(bx - hx + sx, 0, w - 1)];
-    sdx[k] = v.dx;
+    sdx[k] = M == VWB200_OUTLIERS_THRESH && !Px::valid(v) ? Px::absent() : v.dx;
     sdy[k] = v.dy;
-    skey[k] = !Px::valid(v) ? kNoKeyO : M == VWB200_OUTLIERS_MEAN ? Px::key(v.dx, v.dy) : 0u;
+    if (M != VWB200_OUTLIERS_THRESH) skey[k] = !Px::valid(v) ? kNoKeyO : M == VWB200_OUTLIERS_MEAN ? Px::key(v.dx, v.dy) : 0u;
   }
   __syncthreads();
   const int ox = blockIdx.x * RO_TW + threadIdx.x, oy = blockIdx.y * RO_TH + threadIdx.y;
@@ -224,7 +179,7 @@ outlier_pass1_kernel(const T* __restrict__ in, int w, int h, ptrdiff_t ipitch, i
       for (int yk = 0; yk <= 2 * hy; ++yk) {
         const int r = base + yk * sw;
         for (int xk = 0; xk <= 2 * hx; ++xk)
-          if (skey[r + xk] != kNoKeyO && Px::absdiff(c.dx, sdx[r + xk]) <= pt && Px::absdiff(c.dy, sdy[r + xk]) <= pt) ++matched;
+          if (Px::present(sdx[r + xk]) && Px::absdiff(c.dx, sdx[r + xk]) <= pt && Px::absdiff(c.dy, sdy[r + xk]) <= pt) ++matched;
       }
       reject = __ddiv_rn((double)matched, (double)((2 * hx + 1) * (2 * hy + 1))) < rt;
     } else if (M == VWB200_OUTLIERS_MEAN) {               // :497-550
@@ -321,7 +276,8 @@ int outlier_pass1_launch(int method, const T* in, int w, int h, ptrdiff_t ipitch
     return VWB200_EARG;
   }
   if (ow <= 0 || oh <= 0) return VWB200_OK;
-  const size_t smem = (size_t)(RO_TW + 2 * hx) * (RO_TH + 2 * hy) * 3 * sizeof(unsigned);
+  const size_t planes = method == VWB200_OUTLIERS_THRESH ? 2 : 3;
+  const size_t smem = (size_t)(RO_TW + 2 * hx) * (RO_TH + 2 * hy) * planes * sizeof(unsigned);
   if (smem > kOutlierSmemMax) { set_error("outlier filter half kernel %dx%d too large", hx, hy); return VWB200_ENOIMPL; }
   const dim3 b(RO_TW, RO_TH), g((ow + RO_TW - 1) / RO_TW, (oh + RO_TH - 1) / RO_TH);
   if (g.y > 65535) { set_error("outlier filter: %d rows are above the supported %d", oh, 65535 * RO_TH); return VWB200_ENOIMPL; }
@@ -329,7 +285,7 @@ int outlier_pass1_launch(int method, const T* in, int w, int h, ptrdiff_t ipitch
       method == VWB200_OUTLIERS_THRESH ? outlier_pass1_kernel<T, VWB200_OUTLIERS_THRESH>
       : method == VWB200_OUTLIERS_MEAN ? outlier_pass1_kernel<T, VWB200_OUTLIERS_MEAN>
                                        : outlier_pass1_kernel<T, VWB200_OUTLIERS_STDDEV>;
-  VWB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  VWB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));   // per-function state shared by all host threads: device maximum
   kern<<<g, b, smem, st>>>(in, w, h, ipitch, hx, hy, pt, rt, max_mean_diff * max_mean_diff, x0, y0, ow, oh, out, opitch);
   VWB_LAUNCH_CHECK();
   return VWB200_OK;
