@@ -211,6 +211,30 @@ int vwb200_transform_image(const vwb200_warp_params* p, const float* in, int w, 
                            void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * fill_holes_grass(img, hole_fill_len) (src/vw/Image/InpaintView.h:239-311) of a disparity (VWB200_DISP_I32 /
+ * VWB200_DISP_F32), rasterised over the output window (x0, y0, ow, oh), which must lie inside the w x h input.  As in the
+ * reference, the result depends on the window: the holes are looked for in the window grown by hole_fill_len (and cropped to
+ * the image).  A hole is an 8-connected component of invalid pixels; it is filled when its bounding box is at most
+ * hole_fill_len wide and tall, and its bounding box grown by one pixel lies inside that tile with its last column / row below
+ * cols - 1 / rows - 1 (InpaintView.h:76-80 tests max >= cols on a half-open box, so a hole reaching column cols - 2 is
+ * skipped too).  Its pixels are then ordered by their city-block distance to the nearest non-hole pixel, then column-major,
+ * and given 10 * max_distance^2 in-place sweeps of the 8-neighbour stencil (.176765 corners, .073235 edges; each product in
+ * double, each sum rounded to float; int32 stores truncate).  The first sweep reads the holes' invalid children as they are.
+ * Filled pixels get valid = 1; every other pixel is copied, valid word included.  hole_fill_len = 0 fills nothing.
+ * Exactness: bit for bit the reference's (floats as raw bits, NaN payloads not kept); int32 children need |dx|, |dy| < 2^30.
+ * VWB200_EARG, before the device is looked up, for a NULL in / out, an unknown pixel type, w, h, ow, oh <= 0, a pitch below its
+ * width, a window outside the input, and, where the reference does not check, for hole_fill_len < 0, a hole_fill_len^2 that
+ * overflows int32, and an out that overlaps in.  VWB200_ENOIMPL for a tile of 2^30 pixels or more.
+ * vwb200_last_fill_stats reports the last call on this thread: holes found in the tile, holes filled (those that meet the
+ * window), the largest 10 * max_distance^2, the most levels of one hole and the longest chain of synchronised steps
+ * (sweeps x levels) of one hole.
+ * ------------------------------------------------------------------------------------------- */
+int vwb200_fill_holes_grass(int pixel_type, const void* in, int w, int h, ptrdiff_t pitch, int hole_fill_len, int x0, int y0, void* out,
+                            int ow, int oh, ptrdiff_t opitch, int on_device, void* stream);
+typedef struct { long long holes, filled, max_sweeps, max_levels, critical_steps; } vwb200_fill_stats;
+int vwb200_last_fill_stats(vwb200_fill_stats* out);
+
+/* ---------------------------------------------------------------------------------------------
  * vw::stereo::ParabolaSubpixelView::rasterize(dest, bbox) (src/vw/Stereo/ParabolaSubpixelView.h:27-117,
  * .cc:31-330): 3x3 AbsoluteCost patch around the integer disparity, 6x9 pseudo-inverse parabola fit,
  * offset kept when its norm is below 5.  disparity: cols x rows PixelMask<Vector2f> triples (same size as

@@ -17,6 +17,8 @@ Names, argument order and error behaviour follow Vision Workbench:
                               -- src/vw/Stereo/DisparityMap.h:48-66, 255-300, 1016-1057, 1190-1224, 1251-1358
   * transform with HomographyTransform / DisparityTransform (float32 images; bilinear, bicubic, nearest; zero or
     constant edges)           -- src/vw/Image/Transform.h:485-601, Math/Transform.h:369-389, Stereo/DisparityMap.h:1164-1187
+  * fill_holes_grass (int32 or float32 disparities)
+                              -- src/vw/Image/InpaintView.h:239-311
 
 There is no CPU path: every call goes to libvwb200.so (hand-written sm_90a kernels) and raises if
 the library or a CUDA device is missing.  Inputs may be numpy arrays (staged through HBM by the
@@ -133,6 +135,8 @@ def lib():
         L.vwb200_disparity_range_mask.argtypes = [I, P, I, I, Z, P, P, P, Z, I, P]
         L.vwb200_transform_disparities.argtypes = [I, I, P, I, P, P, I, I, Z, P, Z, I, P]
         L.vwb200_transform_image.argtypes = [C.POINTER(WarpParams), P, I, I, Z, P, I, I, Z, I, I, P, I, I, Z, I, P]
+        L.vwb200_fill_holes_grass.argtypes = [I, P, I, I, Z, I, I, I, P, I, I, Z, I, P]
+        L.vwb200_last_fill_stats.argtypes = [C.POINTER(FillStats)]
         L.vwb200_corr_create.argtypes = [C.POINTER(CorrParams), C.POINTER(P)]
         L.vwb200_corr_set_inputs.argtypes = [P, P, I, I, Z, P, I, I, Z, P, Z, P, Z, I]
         L.vwb200_corr_rasterize.argtypes = [P, I, I, I, I, P, Z, I, P]
@@ -621,6 +625,34 @@ def transform(image, tx, bbox=None, edge=EDGE_ZERO, interp=INTERP_BILINEAR):
     _check(lib().vwb200_transform_image(C.byref(p), ptr, cols, rows, pitch, dptr, dw, dh, dpitch, x0, y0, _ptr(out), x1 - x0, y1 - y0,
                                         x1 - x0, dev, _stream_ptr() if dev else None))
     return out
+
+
+class FillStats(C.Structure):
+    _fields_ = [("holes", C.c_longlong), ("filled", C.c_longlong), ("max_sweeps", C.c_longlong), ("max_levels", C.c_longlong),
+                ("critical_steps", C.c_longlong)]
+
+
+def fill_holes_grass(disparity_map, hole_fill_len, bbox=None):
+    """fill_holes_grass(img, hole_fill_len) (Image/InpaintView.h:239-311), rasterised over bbox (x0, y0, x1, y1) or a BBox2i
+    inside the image; None is the whole image, the `ImageView<PixelT> result = fill_holes_grass(...)` form.  The holes (8-connected
+    invalid pixels) at most hole_fill_len wide and tall are filled by the grassfire-ordered Gauss-Seidel inpainting of the
+    reference; the result depends on bbox as the reference's does.  int32 or float32 (rows, cols, 3), numpy or CUDA; returns
+    a new (y1 - y0, x1 - x0, 3) raster of the same kind.  ArgumentErr for hole_fill_len < 0 or with hole_fill_len^2 beyond
+    int32, and for a bbox that is empty or leaves the image."""
+    t, ptr, cols, rows, pitch, dev, dt = _disparity_in(disparity_map)
+    x0, y0, x1, y1 = _bbox(bbox) if bbox is not None else (0, 0, cols, rows)
+    out = _output(t, (max(y1 - y0, 0), max(x1 - x0, 0), 3), dt)
+    _check(lib().vwb200_fill_holes_grass(_ptype(dt), ptr, cols, rows, pitch, int(hole_fill_len), x0, y0, _ptr(out), x1 - x0, y1 - y0,
+                                         x1 - x0, dev, _stream_ptr() if dev else None))
+    return out
+
+
+def last_fill_stats():
+    """what the last fill_holes_grass on this thread did: holes found in its tile, holes filled, the largest
+    10 * max_distance^2, the most levels of one hole, and the longest chain of synchronised steps (sweeps x levels)"""
+    s = FillStats()
+    lib().vwb200_last_fill_stats(C.byref(s))
+    return {k: int(getattr(s, k)) for k, _ in FillStats._fields_}
 
 
 def _disparity_arg(disparity):

@@ -226,6 +226,11 @@ template <class T> int dispmap_transform_launch(int mode, const double* m9, int 
 int warp_launch(const vwb200_warp_params& p, const float* in, int w, int h, ptrdiff_t ip, const DispF* disp, int dw, int dh, ptrdiff_t dp,
                 int x0, int y0, float* out, int ow, int oh, ptrdiff_t op, cudaStream_t st);
 
+// ---- K9: fill_holes_grass over an output window (k9_inpaint.cu); T = vwb200_dispi or DispF, pitches in pixels ---------------
+// in and out are device rasters that do not overlap; stats are those of vwb200_last_fill_stats
+template <class T> int fill_holes_grass_launch(const T* in, int w, int h, ptrdiff_t ip, int len, int x0, int y0, T* out, int ow, int oh,
+                                               ptrdiff_t op, Arena& ar, cudaStream_t st, vwb200_fill_stats* stats);
+
 // ---- host-side restatement-free logic -----------------------------------------------------------
 struct Box { int x0, y0, x1, y1; };
 struct HostZone { Box img; Box disp; };

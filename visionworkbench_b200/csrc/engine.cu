@@ -942,6 +942,25 @@ static int outlier_filter_typed(const vwb200_outlier_params& p, const T* in, int
   return c.finish();
 }
 
+// ---- K9: one fill_holes_grass call, staging only the tile it reads --------------------------------------------------------
+static thread_local vwb200_fill_stats t_fill_stats = {0, 0, 0, 0, 0};
+
+template <class T>
+static int fill_holes_typed(const T* in, int w, int h, ptrdiff_t pitch, int len, int x0, int y0, T* out, int ow, int oh, ptrdiff_t opitch,
+                            int on_device, void* stream) {
+  // only the tile (the window grown by len, cropped to the image) is read: stage that alone
+  const int tx0 = (int)std::max<long long>((long long)x0 - len, 0), ty0 = (int)std::max<long long>((long long)y0 - len, 0);
+  const int tx1 = (int)std::min<long long>((long long)x0 + ow + len, w), ty1 = (int)std::min<long long>((long long)y0 + oh + len, h);
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
+  const T* din; ptrdiff_t dp;
+  VWB_TRY(c.in(in + (ptrdiff_t)ty0 * pitch + tx0, tx1 - tx0, ty1 - ty0, pitch, on_device, &din, &dp));
+  T* dout; ptrdiff_t dop;
+  VWB_TRY(c.out((T*)out, ow, oh, opitch, on_device, &dout, &dop));
+  VWB_TRY(fill_holes_grass_launch(din, tx1 - tx0, ty1 - ty0, dp, len, x0 - tx0, y0 - ty0, dout, ow, oh, dop, c.ar, c.st, &t_fill_stats));
+  return c.finish();
+}
+
 // ---- K7: resampling, range and transforms of a disparity (Stereo/DisparityMap.h) ----------------------------------------------
 // the argument checks every K7 call shares; `what` names the call in the messages
 static int dispmap_check(const char* what, int pixel_type, const void* in, int w, int h, ptrdiff_t pitch) {
@@ -1651,6 +1670,32 @@ int vwb200_transform_image(const vwb200_warp_params* p, const float* in, int w, 
   VWB_TRY(c.out(out, ow, oh, opitch, on_device, &dout, &dop));
   VWB_TRY(warp_launch(*p, din, w, h, dp, dd, dw, dh, ddp, x0, y0, dout, ow, oh, dop, c.st));
   return c.finish();
+}
+
+// ---- K9: fill_holes_grass (Image/InpaintView.h:239-311) -------------------------------------------------------------------
+int vwb200_last_fill_stats(vwb200_fill_stats* out) { if (!out) return VWB200_EARG; *out = t_fill_stats; return VWB200_OK; }
+
+int vwb200_fill_holes_grass(int pixel_type, const void* in, int w, int h, ptrdiff_t pitch, int hole_fill_len, int x0, int y0, void* out,
+                            int ow, int oh, ptrdiff_t opitch, int on_device, void* stream) {
+  t_fill_stats = vwb200_fill_stats{0, 0, 0, 0, 0};
+  if (!in || !out) { set_error("fill_holes_grass: null input or output"); return VWB200_EARG; }
+  if (pixel_type != VWB200_DISP_I32 && pixel_type != VWB200_DISP_F32) { set_error("fill_holes_grass: unknown pixel type %d", pixel_type); return VWB200_EARG; }
+  if (hole_fill_len < 0) { set_error("fill_holes_grass: hole_fill_len %d is negative", hole_fill_len); return VWB200_EARG; }
+  if ((long long)hole_fill_len * hole_fill_len > INT_MAX) {       // InpaintView.h:276 computes len * len in int
+    set_error("fill_holes_grass: hole_fill_len %d squared overflows int32", hole_fill_len);
+    return VWB200_EARG;
+  }
+  if (w <= 0 || h <= 0 || pitch < w) { set_error("fill_holes_grass: bad input size %d x %d, pitch %td", w, h, pitch); return VWB200_EARG; }
+  if (ow <= 0 || oh <= 0 || opitch < ow) { set_error("fill_holes_grass: bad output size %d x %d, pitch %td", ow, oh, opitch); return VWB200_EARG; }
+  if (x0 < 0 || y0 < 0 || x0 > w - ow || y0 > h - oh) {
+    set_error("fill_holes_grass: the window (%d, %d, %d, %d) leaves the %d x %d input", x0, y0, ow, oh, w, h);
+    return VWB200_EARG;
+  }
+  if (rasters_overlap(in, w, h, pitch, out, ow, oh, opitch)) { set_error("fill_holes_grass: out overlaps in"); return VWB200_EARG; }
+  VWB_TRY(ensure_device());
+  if (pixel_type == VWB200_DISP_I32)
+    return fill_holes_typed((const vwb200_dispi*)in, w, h, pitch, hole_fill_len, x0, y0, (vwb200_dispi*)out, ow, oh, opitch, on_device, stream);
+  return fill_holes_typed((const DispF*)in, w, h, pitch, hole_fill_len, x0, y0, (DispF*)out, ow, oh, opitch, on_device, stream);
 }
 
 // ---- the view -------------------------------------------------------------------------------------
