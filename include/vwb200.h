@@ -235,6 +235,62 @@ typedef struct { long long holes, filled, max_sweeps, max_levels, critical_steps
 int vwb200_last_fill_stats(vwb200_fill_stats* out);
 
 /* ---------------------------------------------------------------------------------------------
+ * Dense two-camera triangulation through pinhole cameras (src/vw/Stereo/StereoView.h, StereoModel.cc:35-309,
+ * Camera/PinholeModel.cc:79-116, 422-434, 553-605, Camera/LensDistortion.cc:258-400, Math/NewtonRaphson.cc).
+ * A camera is the parameter list of the PinholeModel constructors: center C, rotation R (row-major), fu, fv, cu, cv, the
+ * u, v, w frame vectors (the unit axes by default), pixel_pitch and a lens distortion: VWB200_LENS_NULL (num_lens_params 0)
+ * or VWB200_LENS_TSAI (num_lens_params 5: k1, k2, p1, p2, k3).  Per call the host builds the inverse camera transform
+ * inverse(uvw * transpose(R)) * inverse(K) exactly as rebuild_camera_matrix does (LU with partial pivoting, Math/Matrix.h:
+ * 2218-2281); a u, v, w frame that fails its orthonormality asserts is VWB200_ELOGIC, a singular matrix VWB200_EMATH.
+ * Per pixel: pixel_to_vector of both pixels (undistort pix * pixel_pitch -- Tsai by Newton-Raphson, tol 1e-9, at most 19
+ * iterations --, inv * (u, v, 1), normalised), the nearly-parallel test 1 - dot(d0, d1) >= tol (tol = angle_tol when
+ * angle_tol > 0, else 1e-4; NaN directions count as parallel), the closest-point midpoint and its reflection through cam1's center
+ * when it falls behind either camera.  A pixel with a NaN component or equal to (-1e8, -1e8) is skipped; with a ray skipped or
+ * parallel rays the point is (0, 0, 0).  Exactness: every double bit for bit the reference's (NaN payloads not kept).
+ * Points are {x, y, z} doubles (24 bytes), pitches in pixels.  VWB200_EARG, before the device is looked up, for a NULL
+ * pointer, an unknown pixel type or lens, w, h, ow, oh <= 0, a pitch below its width, a window outside the input, a Tsai lens
+ * without num_lens_params == 5, a NULL lens with parameters, and an output that overlaps an input.
+ * ------------------------------------------------------------------------------------------- */
+enum { VWB200_LENS_NULL = 0, VWB200_LENS_TSAI = 1 };
+typedef struct {
+  double center[3];
+  double rotation[9];
+  double fu, fv, cu, cv;
+  double u_direction[3], v_direction[3], w_direction[3];
+  double pixel_pitch;
+  int lens;                 /* VWB200_LENS_* */
+  int num_lens_params;      /* 0 for NULL, 5 for TSAI */
+  double lens_params[5];    /* TSAI: k1, k2, p1, p2, k3 */
+} vwb200_pinhole;
+
+/* stereo_triangulate(disparity, cam1, cam2) (StereoView.h:74-130) rasterised over the window (x0, y0, ow, oh) of a w x h
+ * disparity (VWB200_DISP_I32 / VWB200_DISP_F32): pixel (i, j) triangulates (i, j) against (i, j) + (double)disparity;
+ * an invalid pixel (valid == 0) gives (0, 0, 0).  xyz is ow x oh. */
+int vwb200_stereo_triangulate(int pixel_type, const void* disparity, int w, int h, ptrdiff_t pitch, int x0, int y0, int ow, int oh,
+                              const vwb200_pinhole* cam1, const vwb200_pinhole* cam2, double angle_tol, double* xyz, ptrdiff_t xyz_pitch,
+                              int on_device, void* stream);
+/* StereoModel::operator()(ImageView<PixelMask<Vector2f>>, ImageView<double>& error) (StereoModel.cc:254-309) over a whole
+ * w x h float disparity: pixel (x, y) triangulates (x, y) against (x + dx, y + dy) summed in float; error = norm_2 of the
+ * closest points' difference.  An invalid pixel gives xyz 0 and error 0; a NaN error gives xyz 0, keeps the NaN and counts
+ * as divergent. */
+int vwb200_stereo_model_points(const float* disparity, int w, int h, ptrdiff_t pitch, const vwb200_pinhole* cam1,
+                               const vwb200_pinhole* cam2, double angle_tol, double* xyz, ptrdiff_t xyz_pitch, double* error,
+                               ptrdiff_t error_pitch, int on_device, void* stream);
+/* what the last vwb200_stereo_model_points on this thread reports (StereoModel.cc:301-307): points with error >= 0, divergent
+ * points, the largest error (exact) and the sum of the errors (summed in another order than the reference's raster order:
+ * within 1e-12 relative); the mean error is error_sum / points.  tsai_iterations: the Newton-Raphson iterations of the last
+ * vwb200_stereo_triangulate or vwb200_stereo_model_points (both rays of every triangulated pixel). */
+typedef struct { long long points, divergent; double max_error, error_sum; long long tsai_iterations; } vwb200_triangulation_stats;
+int vwb200_last_triangulation_stats(vwb200_triangulation_stats* out);
+/* UniverseRadiusFunc(origin, near_radius, far_radius) applied to a w x h Vector3 image (StereoView.h:139-186): a point equal to
+ * (0, 0, 0) (-0.0 included) becomes +0 and is not rejected; otherwise dist = norm_2(p - origin), and the point becomes +0
+ * and is rejected when (near != 0 && dist < near) || (far != 0 && dist > far); a NaN point passes unchanged.  out may be in
+ * (same pitch).  *rejected / *total (may be NULL) receive the counts.  VWB200_EARG also for radii that are not >= 0 or
+ * near > far (the reference's asserts); far = DBL_MAX is the reference's default. */
+int vwb200_universe_radius(const double* in, int w, int h, ptrdiff_t pitch, const double origin[3], double near_radius, double far_radius,
+                           double* out, ptrdiff_t out_pitch, long long* rejected, long long* total, int on_device, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * vw::stereo::ParabolaSubpixelView::rasterize(dest, bbox) (src/vw/Stereo/ParabolaSubpixelView.h:27-117,
  * .cc:31-330): 3x3 AbsoluteCost patch around the integer disparity, 6x9 pseudo-inverse parabola fit,
  * offset kept when its norm is below 5.  disparity: cols x rows PixelMask<Vector2f> triples (same size as

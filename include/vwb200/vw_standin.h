@@ -13,7 +13,11 @@
 //   vw::rasterize               Image/ImageViewBase.h:283-316
 //   Exception hierarchy         Core/Exception.h:201-253
 //   Zero/ConstantEdgeExtension, Bilinear/Bicubic/NearestPixelInterpolation   tag types only (EdgeExtension.tcc, Interpolation.h)
+//   Vector3                     Math/Vector.h           (3 doubles)
+//   camera::CameraModel, PinholeModel, NullLensDistortion, TsaiLensDistortion
+//                               Camera/CameraModel.h, PinholeModel.h:158-261, LensDistortion.h (constructors and accessors only)
 #pragma once
+#include <vector>
 #include <cstddef>
 #include <cstdint>
 #include <cstring>
@@ -57,6 +61,15 @@ template <class T> struct Vector2 {
 };
 typedef Vector2<int32> Vector2i;
 typedef Vector2<float> Vector2f;
+
+struct Vector3 {                                                                        // Vector<double, 3>
+  double v[3];
+  Vector3() { v[0] = v[1] = v[2] = 0.0; }
+  Vector3(double a, double b, double c) { v[0] = a; v[1] = b; v[2] = c; }
+  double& operator[](size_t i) { return v[i]; }
+  double const& operator[](size_t i) const { return v[i]; }
+};
+static_assert(sizeof(Vector3) == 24, "Vector3 must be 3 doubles");
 
 class BBox2i {
   Vector2i m_min, m_max;
@@ -209,6 +222,60 @@ public:
   ProceduralPixelAccessor& advance(int32 dc, int32 dr, ptrdiff_t dp = 0) { m_c += dc; m_r += dr; m_p += int32(dp); return *this; }
   result_type operator*() const { return m_view(m_c, m_r, m_p); }
 };
+
+namespace camera {
+class CameraModel {                                                                           // Camera/CameraModel.h:62-102
+public:
+  virtual ~CameraModel() {}
+  virtual std::string type() const = 0;
+};
+class LensDistortion {                                                                        // Camera/LensDistortion.h:44-100
+public:
+  virtual ~LensDistortion() {}
+  virtual std::vector<double> distortion_parameters() const { return std::vector<double>(); }
+  virtual std::string name() const = 0;
+  virtual LensDistortion* copy() const = 0;
+};
+class NullLensDistortion : public LensDistortion {
+public:
+  std::string name() const override { return "NULL"; }
+  LensDistortion* copy() const override { return new NullLensDistortion(*this); }
+};
+class TsaiLensDistortion : public LensDistortion {                                            // k1, k2, p1, p2, k3
+  std::vector<double> m_distortion;
+public:
+  explicit TsaiLensDistortion(std::vector<double> const& params) : m_distortion(params) {
+    if (m_distortion.size() != 5) vw_throw(IOErr() << "TsaiLensDistortion: Incorrect number of parameters was passed in.");
+  }
+  std::vector<double> distortion_parameters() const override { return m_distortion; }
+  std::string name() const override { return "TSAI"; }
+  LensDistortion* copy() const override { return new TsaiLensDistortion(*this); }
+};
+class PinholeModel : public CameraModel {                                                      // Camera/PinholeModel.cc:79-116
+  Vector3 m_center, m_u, m_v, m_w;
+  Matrix3x3 m_rotation;
+  double m_fu, m_fv, m_cu, m_cv, m_pixel_pitch;
+  std::shared_ptr<LensDistortion> m_distortion;
+public:
+  PinholeModel(Vector3 camera_center, Matrix3x3 rotation, double f_u, double f_v, double c_u, double c_v, Vector3 u_direction,
+               Vector3 v_direction, Vector3 w_direction, LensDistortion const* distortion_model = 0, double pixel_pitch = 1.0)
+    : m_center(camera_center), m_u(u_direction), m_v(v_direction), m_w(w_direction), m_rotation(rotation), m_fu(f_u), m_fv(f_v),
+      m_cu(c_u), m_cv(c_v), m_pixel_pitch(pixel_pitch),
+      m_distortion(distortion_model ? distortion_model->copy() : new NullLensDistortion) {}
+  PinholeModel(Vector3 camera_center, Matrix3x3 rotation, double f_u, double f_v, double c_u, double c_v,
+               LensDistortion const* distortion_model = 0, double pixel_pitch = 1.0)
+    : PinholeModel(camera_center, rotation, f_u, f_v, c_u, c_v, Vector3(1, 0, 0), Vector3(0, 1, 0), Vector3(0, 0, 1), distortion_model,
+                   pixel_pitch) {}
+  std::string type() const override { return "Pinhole"; }
+  Vector3 camera_center(Vector2<double> const& = Vector2<double>()) const { return m_center; }
+  Matrix3x3 const& get_rotation_matrix() const { return m_rotation; }
+  Vector2<double> focal_length() const { return Vector2<double>(m_fu, m_fv); }
+  Vector2<double> point_offset() const { return Vector2<double>(m_cu, m_cv); }
+  void coordinate_frame(Vector3& u, Vector3& v, Vector3& w) const { u = m_u; v = m_v; w = m_w; }
+  double pixel_pitch() const { return m_pixel_pitch; }
+  LensDistortion const* lens_distortion() const { return m_distortion.get(); }
+};
+}  // namespace camera
 
 namespace stereo {
 struct SemiGlobalMatcher {                                                                    // Stereo/SGM.h:93-99

@@ -19,6 +19,8 @@ Names, argument order and error behaviour follow Vision Workbench:
     constant edges)           -- src/vw/Image/Transform.h:485-601, Math/Transform.h:369-389, Stereo/DisparityMap.h:1164-1187
   * fill_holes_grass (int32 or float32 disparities)
                               -- src/vw/Image/InpaintView.h:239-311
+  * PinholeModel (NULL or TSAI lens), stereo_triangulate, stereo_model_points (StereoModel::operator() on an image),
+    universe_radius           -- src/vw/Camera/PinholeModel.cc:79-116, Stereo/StereoView.h:74-186, StereoModel.cc:254-309
 
 There is no CPU path: every call goes to libvwb200.so (hand-written sm_90a kernels) and raises if
 the library or a CUDA device is missing.  Inputs may be numpy arrays (staged through HBM by the
@@ -137,6 +139,10 @@ def lib():
         L.vwb200_transform_image.argtypes = [C.POINTER(WarpParams), P, I, I, Z, P, I, I, Z, I, I, P, I, I, Z, I, P]
         L.vwb200_fill_holes_grass.argtypes = [I, P, I, I, Z, I, I, I, P, I, I, Z, I, P]
         L.vwb200_last_fill_stats.argtypes = [C.POINTER(FillStats)]
+        L.vwb200_stereo_triangulate.argtypes = [I, P, I, I, Z, I, I, I, I, C.POINTER(Pinhole), C.POINTER(Pinhole), D, P, Z, I, P]
+        L.vwb200_stereo_model_points.argtypes = [P, I, I, Z, C.POINTER(Pinhole), C.POINTER(Pinhole), D, P, Z, P, Z, I, P]
+        L.vwb200_last_triangulation_stats.argtypes = [C.POINTER(TriangulationStats)]
+        L.vwb200_universe_radius.argtypes = [P, I, I, Z, P, D, D, P, Z, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong), I, P]
         L.vwb200_corr_create.argtypes = [C.POINTER(CorrParams), C.POINTER(P)]
         L.vwb200_corr_set_inputs.argtypes = [P, P, I, I, Z, P, I, I, Z, P, Z, P, Z, I]
         L.vwb200_corr_rasterize.argtypes = [P, I, I, I, I, P, Z, I, P]
@@ -653,6 +659,123 @@ def last_fill_stats():
     s = FillStats()
     lib().vwb200_last_fill_stats(C.byref(s))
     return {k: int(getattr(s, k)) for k, _ in FillStats._fields_}
+
+
+LENS_NULL, LENS_TSAI = 0, 1
+DBL_MAX = float(np.finfo(np.float64).max)
+
+
+class Pinhole(C.Structure):
+    _fields_ = [("center", C.c_double * 3), ("rotation", C.c_double * 9), ("fu", C.c_double), ("fv", C.c_double), ("cu", C.c_double),
+                ("cv", C.c_double), ("u_direction", C.c_double * 3), ("v_direction", C.c_double * 3), ("w_direction", C.c_double * 3),
+                ("pixel_pitch", C.c_double), ("lens", C.c_int), ("num_lens_params", C.c_int), ("lens_params", C.c_double * 5)]
+
+
+class TsaiLensDistortion:
+    """TsaiLensDistortion(params) (Camera/LensDistortion.h): k1, k2, p1, p2, k3"""
+
+    def __init__(self, params):
+        self.params = tuple(float(p) for p in params)
+        if len(self.params) != 5:
+            raise ArgumentErr("TsaiLensDistortion: Incorrect number of parameters was passed in.")
+
+    def name(self):
+        return "TSAI"
+
+
+class NullLensDistortion:
+    def name(self):
+        return "NULL"
+
+
+class PinholeModel:
+    """camera::PinholeModel(camera_center, rotation, f_u, f_v, c_u, c_v[, u_direction, v_direction, w_direction],
+    distortion_model=None, pixel_pitch=1.0) (Camera/PinholeModel.cc:79-116): the parameters only; the engine builds the inverse
+    camera transform of each call from them, as rebuild_camera_matrix does.  distortion_model: None / NullLensDistortion() or
+    TsaiLensDistortion(k1, k2, p1, p2, k3)."""
+
+    def __init__(self, camera_center, rotation, f_u, f_v, c_u, c_v, u_direction=(1, 0, 0), v_direction=(0, 1, 0), w_direction=(0, 0, 1),
+                 distortion_model=None, pixel_pitch=1.0):
+        self.camera_center = tuple(float(x) for x in camera_center)
+        self.rotation = np.asarray(rotation, np.float64).reshape(3, 3).copy()
+        self.fu, self.fv, self.cu, self.cv = float(f_u), float(f_v), float(c_u), float(c_v)
+        self.frame = tuple(tuple(float(x) for x in d) for d in (u_direction, v_direction, w_direction))
+        self.distortion = distortion_model if distortion_model is not None else NullLensDistortion()
+        self.pixel_pitch = float(pixel_pitch)
+
+    def _struct(self):
+        p = Pinhole()
+        p.center[:] = self.camera_center
+        p.rotation[:] = [float(x) for x in self.rotation.reshape(9)]
+        p.fu, p.fv, p.cu, p.cv = self.fu, self.fv, self.cu, self.cv
+        p.u_direction[:], p.v_direction[:], p.w_direction[:] = self.frame
+        p.pixel_pitch = self.pixel_pitch
+        if isinstance(self.distortion, TsaiLensDistortion):
+            p.lens, p.num_lens_params = LENS_TSAI, 5
+            p.lens_params[:] = self.distortion.params
+        elif not isinstance(self.distortion, NullLensDistortion):
+            raise NoImplErr(f"lens distortion {self.distortion.name()} has no device form (NULL and TSAI do)")
+        return p
+
+
+def stereo_triangulate(disparity, cam1, cam2, bbox=None, angle_tol=0.0):
+    """stereo_triangulate(disparity, cam1, cam2) (Stereo/StereoView.h:74-130) rasterised over bbox (x0, y0, x1, y1) or a BBox2i
+    inside the image (None: the whole image).  Pixel (i, j) triangulates (i, j) against (i, j) + (double)disparity through
+    StereoModel(cam1, cam2, angle_tol); invalid pixels give (0, 0, 0).  int32 or float32 (rows, cols, 3), numpy or CUDA;
+    returns a (y1 - y0, x1 - x0, 3) float64 raster of the same kind."""
+    t, ptr, cols, rows, pitch, dev, dt = _disparity_in(disparity)
+    x0, y0, x1, y1 = _bbox(bbox) if bbox is not None else (0, 0, cols, rows)
+    out = _output(t, (max(y1 - y0, 0), max(x1 - x0, 0), 3), np.float64)
+    c1, c2 = cam1._struct(), cam2._struct()
+    _check(lib().vwb200_stereo_triangulate(_ptype(dt), ptr, cols, rows, pitch, x0, y0, x1 - x0, y1 - y0, C.byref(c1), C.byref(c2),
+                                           float(angle_tol), _ptr(out), x1 - x0, dev, _stream_ptr() if dev else None))
+    return out
+
+
+def stereo_model_points(disparity, cam1, cam2, angle_tol=0.0):
+    """StereoModel(cam1, cam2, angle_tol)(disparity_map, error) (Stereo/StereoModel.cc:254-309) of a float32 (rows, cols, 3)
+    disparity, numpy or CUDA: (xyz float64 (rows, cols, 3), error float64 (rows, cols)).  last_triangulation_stats() gives
+    what the reference prints."""
+    t, ptr, cols, rows, pitch, dev, dt = _disparity_in(disparity)
+    if dt != np.float32:
+        raise ArgumentErr("StereoModel takes a float32 (PixelMask<Vector2f>) disparity")
+    xyz, err = _output(t, (rows, cols, 3), np.float64), _output(t, (rows, cols), np.float64)
+    c1, c2 = cam1._struct(), cam2._struct()
+    _check(lib().vwb200_stereo_model_points(ptr, cols, rows, pitch, C.byref(c1), C.byref(c2), float(angle_tol), _ptr(xyz), cols, _ptr(err),
+                                            cols, dev, _stream_ptr() if dev else None))
+    return xyz, err
+
+
+class TriangulationStats(C.Structure):
+    _fields_ = [("points", C.c_longlong), ("divergent", C.c_longlong), ("max_error", C.c_double), ("error_sum", C.c_double),
+                ("tsai_iterations", C.c_longlong)]
+
+
+def last_triangulation_stats():
+    """what the last stereo_model_points on this thread reports: points, divergent, max_error, error_sum (mean error =
+    error_sum / points), and the Tsai Newton-Raphson iterations of the last stereo_triangulate or stereo_model_points"""
+    s = TriangulationStats()
+    lib().vwb200_last_triangulation_stats(C.byref(s))
+    return {k: getattr(s, k) for k, _ in TriangulationStats._fields_}
+
+
+def universe_radius(points, origin, near=0.0, far=DBL_MAX, out=None):
+    """UniverseRadiusFunc(origin, near, far) (Stereo/StereoView.h:139-186) applied to a float64 (rows, cols, 3) point image,
+    numpy or CUDA: (points, rejected, total).  out: None (a new raster) or points itself (in place).  ArgumentErr for
+    radii that are not >= 0 and for near > far, as the reference's asserts."""
+    t, ptr, cols, rows, pitch, dev = _raster(points, np.float64, channels=3)
+    if out is None:
+        out = _output(t, (rows, cols, 3), np.float64)
+        opitch = cols
+    elif out is points and t is points:
+        opitch = pitch
+    else:
+        raise ArgumentErr("out must be None or the points themselves (a dense float64 raster)")
+    o = np.ascontiguousarray(origin, np.float64)
+    rej, tot = C.c_longlong(), C.c_longlong()
+    _check(lib().vwb200_universe_radius(ptr, cols, rows, pitch, o.ctypes.data, float(near), float(far), _ptr(out), opitch, C.byref(rej),
+                                        C.byref(tot), dev, _stream_ptr() if dev else None))
+    return out, rej.value, tot.value
 
 
 def _disparity_arg(disparity):

@@ -231,6 +231,20 @@ int warp_launch(const vwb200_warp_params& p, const float* in, int w, int h, ptrd
 template <class T> int fill_holes_grass_launch(const T* in, int w, int h, ptrdiff_t ip, int len, int x0, int y0, T* out, int ow, int oh,
                                                ptrdiff_t op, Arena& ar, cudaStream_t st, vwb200_fill_stats* stats);
 
+// ---- K10: stereo triangulation (k10_triangulate.cu); pitches in pixels -----------------------------------------------------
+// what PinholeModel::pixel_to_vector and camera_center need, built once per call by the host: the inverse camera transform
+// (row-major), the center, the pixel pitch, the intrinsics the lens normalises by, and the Tsai parameters when tsai != 0
+struct TriCam { double inv[9], c[3], pitch, fu, fv, cu, cv, k[5]; int tsai; };
+// stats: 5 x 8 bytes of zeroed device scratch -- [0] error sum (double), [1] max error (double bits), [2] points,
+// [3] divergent, [4] Tsai Newton-Raphson iterations; form (a) fills [4] only.  xyz pitches count {x, y, z} pixels.
+template <class T> int stereo_triangulate_launch(const T* in, ptrdiff_t ip, int x0, int y0, int ow, int oh, const TriCam& c0, const TriCam& c1,
+                                                 double tol, double* xyz, ptrdiff_t xp, unsigned long long* stats, cudaStream_t st);
+int stereo_model_launch(const DispF* in, int w, int h, ptrdiff_t ip, const TriCam& c0, const TriCam& c1, double tol, double* xyz, ptrdiff_t xp,
+                        double* err, ptrdiff_t ep, unsigned long long* stats, cudaStream_t st);
+// in may be out (same pitch); *rejected (device) is added to
+int universe_radius_launch(const double* in, int w, int h, ptrdiff_t ip, const double* origin, double near_r, double far_r, double* out,
+                           ptrdiff_t op, unsigned long long* rejected, cudaStream_t st);
+
 // ---- host-side restatement-free logic -----------------------------------------------------------
 struct Box { int x0, y0, x1, y1; };
 struct HostZone { Box img; Box disp; };

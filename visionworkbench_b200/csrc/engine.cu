@@ -1698,6 +1698,220 @@ int vwb200_fill_holes_grass(int pixel_type, const void* in, int w, int h, ptrdif
   return fill_holes_typed((const DispF*)in, w, h, pitch, hole_fill_len, x0, y0, (DispF*)out, ow, oh, opitch, on_device, stream);
 }
 
+// ---- K10: triangulation (Stereo/StereoView.h, StereoModel.cc) through pinhole cameras ------------------------------------------
+// The camera is built on the host once per call, in the reference's operation order (x86-64 host code has no FMA to contract
+// into, so every product and sum rounds as the reference's does).
+struct Pt3 { double x, y, z; };
+static thread_local vwb200_triangulation_stats t_tri_stats = {0, 0, 0.0, 0.0, 0};
+
+static double dot3h(const double* a, const double* b) { double r = 0.0; for (int k = 0; k < 3; ++k) r += a[k] * b[k]; return r; }
+
+// vw::math::inverse (Math/Matrix.h:2218-2281) of a 3 x 3 matrix: LU with partial pivoting (the first largest |pivot|), then
+// the lower and upper triangular solves on the permuted identity, in its loop order
+static int lu_inverse3(const double* m, double* inv) {
+  double b[9];
+  std::memcpy(b, m, sizeof b);
+  int pm[3] = {0, 1, 2};
+  for (int i = 0; i < 3; ++i) {
+    int p = i;
+    double mx = -1;
+    for (int k = i; k < 3; ++k)
+      if (std::fabs(b[3 * k + i]) > mx) { mx = std::fabs(b[3 * k + i]); p = k; }
+    if (b[3 * p + i] == 0.0) { set_error("Matrix is singular in inverse()"); return VWB200_EMATH; }
+    if (p != i) {
+      std::swap(pm[i], pm[p]);
+      for (int c = 0; c < 3; ++c) std::swap(b[3 * i + c], b[3 * p + c]);
+    }
+    if (i != 2) {
+      for (int k = i + 1; k < 3; ++k) b[3 * k + i] /= b[3 * i + i];
+      for (int k = i + 1; k < 3; ++k)
+        for (int c = i + 1; c < 3; ++c) b[3 * k + c] -= b[3 * k + i] * b[3 * i + c];
+    }
+  }
+  for (int k = 0; k < 9; ++k) inv[k] = 0.0;
+  for (int i = 0; i < 3; ++i) inv[3 * i + pm[i]] = 1.0;
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) {
+      const double t = inv[3 * i + j];
+      if (t != 0.0)
+        for (int k = i + 1; k < 3; ++k) inv[3 * k + j] -= b[3 * k + i] * t;
+    }
+  for (int i = 2; i >= 0; --i)
+    for (int j = 2; j >= 0; --j) {
+      const double t = inv[3 * i + j] /= b[3 * i + i];
+      if (t != 0.0)
+        for (int k = i - 1; k >= 0; --k) inv[3 * k + j] -= b[3 * k + i] * t;
+    }
+  return VWB200_OK;
+}
+
+// the argument checks of one camera (VWB200_EARG)
+static int pinhole_check(const char* what, const vwb200_pinhole* p) {
+  if (!p) { set_error("%s: null camera", what); return VWB200_EARG; }
+  if (p->lens != VWB200_LENS_NULL && p->lens != VWB200_LENS_TSAI) { set_error("%s: unknown lens distortion %d", what, p->lens); return VWB200_EARG; }
+  const int want = p->lens == VWB200_LENS_TSAI ? 5 : 0;
+  if (p->num_lens_params != want) {
+    set_error("%s: the %s lens distortion takes %d parameters, not %d", what, want ? "TSAI" : "NULL", want, p->num_lens_params);
+    return VWB200_EARG;
+  }
+  return VWB200_OK;
+}
+
+// PinholeModel::rebuild_camera_matrix (PinholeModel.cc:553-605): the orthonormality asserts of u, v, w (VW_LINE_ASSERT throws
+// LogicErr), then m_inv_camera_transform = inverse(uvw * transpose(R)) * inverse(K), each product a dot_prod from 0.0
+static int pinhole_build(const char* what, const vwb200_pinhole& p, TriCam* c) {
+  const double* uvw[3] = {p.u_direction, p.v_direction, p.w_direction};
+  const bool ortho = dot3h(uvw[0], uvw[1]) == 0 && dot3h(uvw[0], uvw[2]) == 0 && dot3h(uvw[1], uvw[2]) == 0 &&
+                     std::fabs(std::sqrt(dot3h(uvw[0], uvw[0])) - 1) < 0.001 && std::fabs(std::sqrt(dot3h(uvw[1], uvw[1])) - 1) < 0.001 &&
+                     std::fabs(std::sqrt(dot3h(uvw[2], uvw[2])) - 1) < 0.001;
+  if (!ortho) { set_error("%s: the u, v, w coordinate frame is not orthonormal", what); return VWB200_ELOGIC; }
+  double m[9], k[9] = {p.fu, 0, p.cu, 0, p.fv, p.cv, 0, 0, 1}, a[9], b[9];
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) m[3 * i + j] = dot3h(uvw[i], p.rotation + 3 * j);       // row i of uvw . column j of R^T
+  VWB_TRY(lu_inverse3(m, a));
+  VWB_TRY(lu_inverse3(k, b));
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) {
+      double r = 0.0;
+      for (int q = 0; q < 3; ++q) r += a[3 * i + q] * b[3 * q + j];
+      c->inv[3 * i + j] = r;
+    }
+  for (int q = 0; q < 3; ++q) c->c[q] = p.center[q];
+  c->pitch = p.pixel_pitch;
+  c->fu = p.fu; c->fv = p.fv; c->cu = p.cu; c->cv = p.cv;
+  for (int q = 0; q < 5; ++q) c->k[q] = p.lens == VWB200_LENS_TSAI ? p.lens_params[q] : 0.0;
+  c->tsai = p.lens == VWB200_LENS_TSAI;
+  return VWB200_OK;
+}
+
+// both cameras, then the device; tol is are_nearly_parallel's (StereoModel.cc:81-83)
+static int cameras_open(const char* what, const vwb200_pinhole* cam1, const vwb200_pinhole* cam2, double angle_tol, TriCam* c0, TriCam* c1,
+                        double* tol) {
+  VWB_TRY(pinhole_build(what, *cam1, c0));
+  VWB_TRY(pinhole_build(what, *cam2, c1));
+  *tol = angle_tol > 0 ? angle_tol : 1e-4;
+  return ensure_device();
+}
+
+// zeroed device statistics of one call, copied to host[5] at finish()
+static int tri_stats_open(AbiCall& c, unsigned long long** d) {
+  VWB_TRY(c.ar.alloc(d, 5));
+  VWB_CUDA(cudaMemsetAsync(*d, 0, 5 * sizeof(unsigned long long), c.st));
+  return VWB200_OK;
+}
+
+int vwb200_last_triangulation_stats(vwb200_triangulation_stats* out) { if (!out) return VWB200_EARG; *out = t_tri_stats; return VWB200_OK; }
+
+int vwb200_stereo_triangulate(int pixel_type, const void* disparity, int w, int h, ptrdiff_t pitch, int x0, int y0, int ow, int oh,
+                              const vwb200_pinhole* cam1, const vwb200_pinhole* cam2, double angle_tol, double* xyz, ptrdiff_t xyz_pitch,
+                              int on_device, void* stream) {
+  t_tri_stats = vwb200_triangulation_stats{0, 0, 0.0, 0.0, 0};
+  const char* what = "stereo_triangulate";
+  if (!disparity || !xyz) { set_error("%s: null disparity or output", what); return VWB200_EARG; }
+  if (pixel_type != VWB200_DISP_I32 && pixel_type != VWB200_DISP_F32) { set_error("%s: unknown pixel type %d", what, pixel_type); return VWB200_EARG; }
+  VWB_TRY(pinhole_check(what, cam1));
+  VWB_TRY(pinhole_check(what, cam2));
+  if (w <= 0 || h <= 0 || pitch < w) { set_error("%s: bad input size %d x %d, pitch %td", what, w, h, pitch); return VWB200_EARG; }
+  if (ow <= 0 || oh <= 0 || xyz_pitch < ow) { set_error("%s: bad output size %d x %d, pitch %td", what, ow, oh, xyz_pitch); return VWB200_EARG; }
+  if (x0 < 0 || y0 < 0 || x0 > w - ow || y0 > h - oh) {
+    set_error("%s: the window (%d, %d, %d, %d) leaves the %d x %d input", what, x0, y0, ow, oh, w, h);
+    return VWB200_EARG;
+  }
+  if (rasters_overlap(disparity, w, h, pitch, xyz, ow, oh, xyz_pitch, 12, 24)) { set_error("%s: xyz overlaps the disparity", what); return VWB200_EARG; }
+  TriCam c0, c1;
+  double tol;
+  VWB_TRY(cameras_open(what, cam1, cam2, angle_tol, &c0, &c1, &tol));
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
+  Pt3* dxyz; ptrdiff_t dxp;
+  VWB_TRY(c.out((Pt3*)xyz, ow, oh, xyz_pitch, on_device, &dxyz, &dxp));
+  unsigned long long* dst;
+  VWB_TRY(tri_stats_open(c, &dst));
+  // only the window is read: stage that alone
+  if (pixel_type == VWB200_DISP_I32) {
+    const vwb200_dispi* din; ptrdiff_t dp;
+    VWB_TRY(c.in((const vwb200_dispi*)disparity + (ptrdiff_t)y0 * pitch + x0, ow, oh, pitch, on_device, &din, &dp));
+    VWB_TRY(stereo_triangulate_launch(din, dp, x0, y0, ow, oh, c0, c1, tol, (double*)dxyz, dxp, dst, c.st));
+  } else {
+    const DispF* din; ptrdiff_t dp;
+    VWB_TRY(c.in((const DispF*)disparity + (ptrdiff_t)y0 * pitch + x0, ow, oh, pitch, on_device, &din, &dp));
+    VWB_TRY(stereo_triangulate_launch(din, dp, x0, y0, ow, oh, c0, c1, tol, (double*)dxyz, dxp, dst, c.st));
+  }
+  unsigned long long s[5];
+  VWB_CUDA(cudaMemcpyAsync(s, dst, sizeof s, cudaMemcpyDeviceToHost, c.st));
+  VWB_TRY(c.finish());
+  t_tri_stats.tsai_iterations = (long long)s[4];
+  return VWB200_OK;
+}
+
+int vwb200_stereo_model_points(const float* disparity, int w, int h, ptrdiff_t pitch, const vwb200_pinhole* cam1,
+                               const vwb200_pinhole* cam2, double angle_tol, double* xyz, ptrdiff_t xyz_pitch, double* error,
+                               ptrdiff_t error_pitch, int on_device, void* stream) {
+  t_tri_stats = vwb200_triangulation_stats{0, 0, 0.0, 0.0, 0};
+  const char* what = "StereoModel";
+  if (!disparity || !xyz || !error) { set_error("%s: null disparity or output", what); return VWB200_EARG; }
+  VWB_TRY(pinhole_check(what, cam1));
+  VWB_TRY(pinhole_check(what, cam2));
+  if (w <= 0 || h <= 0 || pitch < w) { set_error("%s: bad input size %d x %d, pitch %td", what, w, h, pitch); return VWB200_EARG; }
+  if (xyz_pitch < w || error_pitch < w) { set_error("%s: output pitches %td, %td are below the width %d", what, xyz_pitch, error_pitch, w); return VWB200_EARG; }
+  if (rasters_overlap(disparity, w, h, pitch, xyz, w, h, xyz_pitch, 12, 24) || rasters_overlap(disparity, w, h, pitch, error, w, h, error_pitch, 12, 8) ||
+      rasters_overlap(xyz, w, h, xyz_pitch, error, w, h, error_pitch, 24, 8)) {
+    set_error("%s: the disparity, xyz and error rasters overlap", what);
+    return VWB200_EARG;
+  }
+  TriCam c0, c1;
+  double tol;
+  VWB_TRY(cameras_open(what, cam1, cam2, angle_tol, &c0, &c1, &tol));
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
+  const DispF* din; ptrdiff_t dp;
+  VWB_TRY(c.in((const DispF*)disparity, w, h, pitch, on_device, &din, &dp));
+  Pt3* dxyz; ptrdiff_t dxp;
+  VWB_TRY(c.out((Pt3*)xyz, w, h, xyz_pitch, on_device, &dxyz, &dxp));
+  double* derr; ptrdiff_t dep;
+  VWB_TRY(c.out(error, w, h, error_pitch, on_device, &derr, &dep));
+  unsigned long long* dst;
+  VWB_TRY(tri_stats_open(c, &dst));
+  VWB_TRY(stereo_model_launch(din, w, h, dp, c0, c1, tol, (double*)dxyz, dxp, derr, dep, dst, c.st));
+  unsigned long long s[5];
+  VWB_CUDA(cudaMemcpyAsync(s, dst, sizeof s, cudaMemcpyDeviceToHost, c.st));
+  VWB_TRY(c.finish());
+  double sum, mx;
+  std::memcpy(&sum, &s[0], sizeof sum);
+  std::memcpy(&mx, &s[1], sizeof mx);
+  t_tri_stats = vwb200_triangulation_stats{(long long)s[2], (long long)s[3], mx, sum, (long long)s[4]};
+  return VWB200_OK;
+}
+
+int vwb200_universe_radius(const double* in, int w, int h, ptrdiff_t pitch, const double origin[3], double near_radius, double far_radius,
+                           double* out, ptrdiff_t out_pitch, long long* rejected, long long* total, int on_device, void* stream) {
+  const char* what = "UniverseRadius";
+  if (!in || !out || !origin) { set_error("%s: null input, output or origin", what); return VWB200_EARG; }
+  if (w <= 0 || h <= 0 || pitch < w || out_pitch < w) { set_error("%s: bad size %d x %d, pitches %td, %td", what, w, h, pitch, out_pitch); return VWB200_EARG; }
+  if (!(near_radius >= 0 && far_radius >= 0)) { set_error("%s: radii must be >= 0.", what); return VWB200_EARG; }      // StereoView.h:160-163
+  if (!(near_radius <= far_radius)) { set_error("%s: near radius must be <= far radius.", what); return VWB200_EARG; }
+  if (!(out == in && out_pitch == pitch) && rasters_overlap(in, w, h, pitch, out, w, h, out_pitch, 24, 24)) {
+    set_error("%s: out overlaps in (only out == in, with the same pitch, is allowed)", what);
+    return VWB200_EARG;
+  }
+  VWB_TRY(ensure_device());
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
+  const Pt3* din; ptrdiff_t dp;
+  VWB_TRY(c.in((const Pt3*)in, w, h, pitch, on_device, &din, &dp));
+  Pt3* dout; ptrdiff_t dop;
+  VWB_TRY(c.out((Pt3*)out, w, h, out_pitch, on_device, &dout, &dop));
+  unsigned long long* dst;
+  VWB_TRY(tri_stats_open(c, &dst));
+  VWB_TRY(universe_radius_launch((const double*)din, w, h, dp, origin, near_radius, far_radius, (double*)dout, dop, dst, c.st));
+  unsigned long long s[5];
+  VWB_CUDA(cudaMemcpyAsync(s, dst, sizeof s, cudaMemcpyDeviceToHost, c.st));
+  VWB_TRY(c.finish());
+  if (rejected) *rejected = (long long)s[0];
+  if (total) *total = (long long)w * h;
+  return VWB200_OK;
+}
+
 // ---- the view -------------------------------------------------------------------------------------
 int vwb200_corr_create(const vwb200_corr_params* p, vwb200_corr** out) {
   if (!p || !out) { set_error("corr_create: null pointer"); return VWB200_EARG; }
