@@ -43,6 +43,7 @@ extern "C" {
 #define VWB200_ECUDA      -5   /* CUDA runtime failure */
 #define VWB200_ENODEVICE  -6   /* no CUDA device: the engine has no CPU path */
 #define VWB200_ENOMEM     -7
+#define VWB200_EPROJECT   -8   /* -> vw::camera::PointToPixelErr */
 
 /* vw::stereo::CostFunctionType, src/vw/Stereo/CostFunctions.h:143-149 */
 enum { VWB200_ABSOLUTE_DIFFERENCE = 0, VWB200_SQUARED_DIFFERENCE = 1, VWB200_CROSS_CORRELATION = 2,
@@ -289,6 +290,42 @@ int vwb200_last_triangulation_stats(vwb200_triangulation_stats* out);
  * near > far (the reference's asserts); far = DBL_MAX is the reference's default. */
 int vwb200_universe_radius(const double* in, int w, int h, ptrdiff_t pitch, const double origin[3], double near_radius, double far_radius,
                            double* out, ptrdiff_t out_pitch, long long* rejected, long long* total, int on_device, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Epipolar rectification of a pinhole stereo pair (Camera/PinholeModel.cc:351-397, 679-732, Camera/EpipolarUtils.cc:37-76,
+ * Camera/CameraTransform.h:43-183, Image/Transform.h:271-315).  Cameras are vwb200_pinhole as above, NULL or TSAI lens.
+ * point_to_pixel is the reference's with its check on (m_do_point_to_pixel_check): P * (X, 1) de-homogenised, the lens's
+ * distorted_coordinates (TSAI in closed form; HUGE_VAL for fu or fv < 1e-300), / pixel_pitch, then pixel_to_vector of that
+ * pixel against normalize(X - C), retried with their sum; a difference still >= 0.01 or NaN is PointToPixelErr, returned as
+ * VWB200_EPROJECT with the reference's message and the first failing pixel.  Exactness: every double and float bit for bit the
+ * reference's (NaN payloads not kept).  VWB200_EARG comes before the device is looked up; a u, v, w frame that fails the
+ * orthonormality asserts is VWB200_ELOGIC, as are a camera transform's cameras at different centers (the VW_ASSERT of
+ * CameraTransform.h:53).
+ * ------------------------------------------------------------------------------------------- */
+/* epipolar(cam0, cam1, epi0, epi1) on the host: camera_pose() rotations through the quaternion round trip, the baseline as u,
+ * w from the mean look vector, v = w x u, the mean focal length, point offset and pixel pitch, NULL lens and the default
+ * u, v, w frame.  Coincident centers give NaN cameras, as in the reference. */
+int vwb200_pinhole_epipolar(const vwb200_pinhole* cam0, const vwb200_pinhole* cam1, vwb200_pinhole* epi0, vwb200_pinhole* epi1);
+/* resize_epipolar_cameras_to_fit(cam1, cam2, epi1, epi2, roi1, roi2, size1, size2): the BBox2f of each ROI's perimeter
+ * (x0, y0, x1, y1) through CameraTransform(cam, epi)::forward, on the device; both epipolar point offsets shifted by the
+ * smaller minimum corner times epi1's pixel pitch (epi1, epi2 are updated in place); the second pass's bbox maxima truncated
+ * to int32 are the sizes (width, height).  A bound that rounds to zero may carry the other sign of zero than the reference's
+ * order-dependent one; that changes a size or an offset only where the offset itself is +-0. */
+int vwb200_resize_epipolar_cameras_to_fit(const vwb200_pinhole* cam1, const vwb200_pinhole* cam2, vwb200_pinhole* epi1, vwb200_pinhole* epi2,
+                                          const int32_t roi1[4], const int32_t roi2[4], int32_t size1[2], int32_t size2[2], void* stream);
+/* camera_transform(image, src, dst, edge, interp) rasterised over the output window (x0, y0, ow, oh) as vwb200_transform_image
+ * does: out pixel (i, j) is the image interpolated at src.point_to_pixel(dst.pixel_to_vector(p) + C), p = (x0 + i, y0 + j),
+ * with the same interpolations, edges and |c| < 2^30 domain rule.  pixel_type VWB200_PIXEL_GRAY_F32: float pixels, every
+ * interpolation, zero and constant edges.  VWB200_PIXEL_MASK_F32: PixelMask<float> {float value, float valid} pixels (pitches in
+ * pixels), bilinear only, zero ({0, 0}), constant and value edges (VWB200_EDGE_VALUE: ValueEdgeExtension(edge_value
+ * {value, valid})).  The masked arithmetic is the reference's: an integral point returns {value, valid != 0}, an interpolated
+ * one the float value with valid 1 when all four neighbours have valid != 0 (NaN counts as valid) and 0 otherwise; outside the
+ * domain {0, 0}.  Other combinations are VWB200_ENOIMPL.  On VWB200_EPROJECT the contents of out are unspecified. */
+enum { VWB200_PIXEL_GRAY_F32 = 0, VWB200_PIXEL_MASK_F32 = 1 };
+enum { VWB200_EDGE_VALUE = 2 };
+int vwb200_camera_transform(const vwb200_pinhole* src, const vwb200_pinhole* dst, int pixel_type, int interp, int edge, const float edge_value[2],
+                            const void* in, int w, int h, ptrdiff_t pitch, int x0, int y0, void* out, int ow, int oh, ptrdiff_t opitch,
+                            int on_device, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * vw::stereo::ParabolaSubpixelView::rasterize(dest, bbox) (src/vw/Stereo/ParabolaSubpixelView.h:27-117,

@@ -13,9 +13,11 @@
 //   vw::rasterize               Image/ImageViewBase.h:283-316
 //   Exception hierarchy         Core/Exception.h:201-253
 //   Zero/ConstantEdgeExtension, Bilinear/Bicubic/NearestPixelInterpolation   tag types only (EdgeExtension.tcc, Interpolation.h)
+//   ValueEdgeExtension<PixelT>  Image/EdgeExtension.h:66-76 (the edge pixel only)
 //   Vector3                     Math/Vector.h           (3 doubles)
 //   camera::CameraModel, PinholeModel, NullLensDistortion, TsaiLensDistortion
 //                               Camera/CameraModel.h, PinholeModel.h:158-261, LensDistortion.h (constructors and accessors only)
+//   camera::PointToPixelErr     Camera/CameraModel.h:229
 #pragma once
 #include <vector>
 #include <cstddef>
@@ -142,6 +144,7 @@ public:
 };
 template <class C> inline bool is_valid(PixelMask<C> const& p) { return p.valid() != 0; }
 static_assert(sizeof(PixelMask<Vector2f>) == 12, "PixelMask<Vector2f> must be 3 floats (Image/PixelMask.h:52-54)");
+static_assert(sizeof(PixelMask<float>) == 8, "PixelMask<float> must be {value, valid} floats");
 
 // ---- edge extension and interpolation tags (Image/EdgeExtension.tcc:47-94, Image/Interpolation.h:113-225) -----------------
 struct ZeroEdgeExtension {};
@@ -149,6 +152,7 @@ struct ConstantEdgeExtension {};
 struct BilinearInterpolation {};
 struct BicubicInterpolation {};
 struct NearestPixelInterpolation {};
+template <class PixelT> struct ValueEdgeExtension { PixelT m_pix; ValueEdgeExtension(PixelT pix) : m_pix(pix) {} };
 
 // ---- views -------------------------------------------------------------------------------------------
 template <class ImplT> struct ImageViewBase {                     // Image/ImageViewBase.h:57-64
@@ -224,6 +228,7 @@ public:
 };
 
 namespace camera {
+VWB200_STANDIN_EXC(PointToPixelErr);
 class CameraModel {                                                                           // Camera/CameraModel.h:62-102
 public:
   virtual ~CameraModel() {}
@@ -271,6 +276,7 @@ public:
   Matrix3x3 const& get_rotation_matrix() const { return m_rotation; }
   Vector2<double> focal_length() const { return Vector2<double>(m_fu, m_fv); }
   Vector2<double> point_offset() const { return Vector2<double>(m_cu, m_cv); }
+  void set_point_offset(Vector2<double> const& c, bool /*rebuild*/ = true) { m_cu = c[0]; m_cv = c[1]; }
   void coordinate_frame(Vector3& u, Vector3& v, Vector3& w) const { u = m_u; v = m_v; w = m_w; }
   double pixel_pitch() const { return m_pixel_pitch; }
   LensDistortion const* lens_distortion() const { return m_distortion.get(); }

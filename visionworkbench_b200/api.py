@@ -21,6 +21,8 @@ Names, argument order and error behaviour follow Vision Workbench:
                               -- src/vw/Image/InpaintView.h:239-311
   * PinholeModel (NULL or TSAI lens), stereo_triangulate, stereo_model_points (StereoModel::operator() on an image),
     universe_radius           -- src/vw/Camera/PinholeModel.cc:79-116, Stereo/StereoView.h:74-186, StereoModel.cc:254-309
+  * epipolar, resize_epipolar_cameras_to_fit, camera_transform, epipolar_transformed_images (float32 or PixelMask<float>
+    images)                   -- src/vw/Camera/PinholeModel.cc:351-397, 679-732, EpipolarUtils.cc:37-144, CameraTransform.h
 
 There is no CPU path: every call goes to libvwb200.so (hand-written sm_90a kernels) and raises if
 the library or a CUDA device is missing.  Inputs may be numpy arrays (staged through HBM by the
@@ -73,7 +75,11 @@ class NoDeviceErr(VwError):
     pass
 
 
-_ERR = {-1: ArgumentErr, -2: MathErr, -3: LogicErr, -4: NoImplErr, -5: CudaErr, -6: NoDeviceErr, -7: MemoryError}
+class PointToPixelErr(VwError):
+    """vw::camera::PointToPixelErr: point_to_pixel's round-trip check failed (VWB200_EPROJECT)"""
+
+
+_ERR = {-1: ArgumentErr, -2: MathErr, -3: LogicErr, -4: NoImplErr, -5: CudaErr, -6: NoDeviceErr, -7: MemoryError, -8: PointToPixelErr}
 
 
 class CorrParams(C.Structure):
@@ -143,6 +149,10 @@ def lib():
         L.vwb200_stereo_model_points.argtypes = [P, I, I, Z, C.POINTER(Pinhole), C.POINTER(Pinhole), D, P, Z, P, Z, I, P]
         L.vwb200_last_triangulation_stats.argtypes = [C.POINTER(TriangulationStats)]
         L.vwb200_universe_radius.argtypes = [P, I, I, Z, P, D, D, P, Z, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong), I, P]
+        PH = C.POINTER(Pinhole)
+        L.vwb200_pinhole_epipolar.argtypes = [PH, PH, PH, PH]
+        L.vwb200_resize_epipolar_cameras_to_fit.argtypes = [PH, PH, PH, PH, P, P, P, P, P]
+        L.vwb200_camera_transform.argtypes = [PH, PH, I, I, I, P, P, I, I, Z, I, I, P, I, I, Z, I, P]
         L.vwb200_corr_create.argtypes = [C.POINTER(CorrParams), C.POINTER(P)]
         L.vwb200_corr_set_inputs.argtypes = [P, P, I, I, Z, P, I, I, Z, P, Z, P, Z, I]
         L.vwb200_corr_rasterize.argtypes = [P, I, I, I, I, P, Z, I, P]
@@ -581,7 +591,7 @@ def _transform(mode, matrix, do_round, box, disparity_map, out):
 # vwb200_transform_image's transform kinds, interpolations and edge extensions (include/vwb200.h)
 WARP_HOMOGRAPHY, WARP_DISPARITY = 0, 1
 INTERP_BILINEAR, INTERP_BICUBIC, INTERP_NEAREST = 0, 1, 2
-EDGE_ZERO, EDGE_CONSTANT = 0, 1
+EDGE_ZERO, EDGE_CONSTANT, EDGE_VALUE = 0, 1, 2   # EDGE_VALUE: ValueEdgeExtension, camera_transform of PixelMask<float> images
 
 
 class WarpParams(C.Structure):
@@ -716,6 +726,12 @@ class PinholeModel:
         elif not isinstance(self.distortion, NullLensDistortion):
             raise NoImplErr(f"lens distortion {self.distortion.name()} has no device form (NULL and TSAI do)")
         return p
+
+    @classmethod
+    def _from_struct(cls, p):
+        lens = TsaiLensDistortion(p.lens_params[:]) if p.lens == LENS_TSAI else None
+        return cls(p.center[:], np.array(p.rotation[:]).reshape(3, 3), p.fu, p.fv, p.cu, p.cv, p.u_direction[:], p.v_direction[:],
+                   p.w_direction[:], lens, p.pixel_pitch)
 
 
 def stereo_triangulate(disparity, cam1, cam2, bbox=None, angle_tol=0.0):
@@ -989,3 +1005,69 @@ def pyramid_correlate(left, right, left_mask, right_mask, prefilter_mode, prefil
                                   min_consistency_level, filter_half_kernel, max_pyramid_levels, algorithm,
                                   collar_size, sgm_subpixel_mode, sgm_search_buffer, memory_limit_mb, blob_filter_area,
                                   lr_disp_diff, region_ul, write_debug_images, **kw)
+
+
+PIXEL_GRAY_F32, PIXEL_MASK_F32 = 0, 1
+
+
+def epipolar(cam0, cam1):
+    """epipolar(cam0, cam1, epi0, epi1) (Camera/PinholeModel.cc:679-732): two rectified PinholeModels at the sources' centers,
+    sharing one rotation (baseline as u), the mean focal length, point offset and pixel pitch, the NULL lens and the default
+    u, v, w frame.  Host arithmetic, bit for bit the reference's; coincident centers give NaN cameras."""
+    a, b = Pinhole(), Pinhole()
+    _check(lib().vwb200_pinhole_epipolar(C.byref(cam0._struct()), C.byref(cam1._struct()), C.byref(a), C.byref(b)))
+    return PinholeModel._from_struct(a), PinholeModel._from_struct(b)
+
+
+def _roi(r):
+    return (C.c_int32 * 4)(*_bbox(r))
+
+
+def resize_epipolar_cameras_to_fit(cam1, cam2, epi1, epi2, roi1, roi2):
+    """resize_epipolar_cameras_to_fit (Camera/EpipolarUtils.cc:37-76): (epi1, epi2, size1, size2) -- new epipolar cameras whose
+    point offsets put both transformed ROIs (x0, y0, x1, y1) or BBox2i at (0, 0), and the (width, height) that holds each.
+    The ROI perimeters go through CameraTransform(cam, epi)::forward on the device.  PointToPixelErr where the reference throws,
+    LogicErr for a camera and its epipolar camera at different centers."""
+    e1, e2 = epi1._struct(), epi2._struct()
+    s1, s2 = (C.c_int32 * 2)(), (C.c_int32 * 2)()
+    _check(lib().vwb200_resize_epipolar_cameras_to_fit(C.byref(cam1._struct()), C.byref(cam2._struct()), C.byref(e1), C.byref(e2), _roi(roi1),
+                                                      _roi(roi2), s1, s2, None))
+    return PinholeModel._from_struct(e1), PinholeModel._from_struct(e2), (s1[0], s1[1]), (s2[0], s2[1])
+
+
+def camera_transform(image, src_camera, dst_camera, bbox=None, size=None, edge=EDGE_ZERO, interp=INTERP_BILINEAR, edge_value=None):
+    """camera_transform(image, src_camera, dst_camera[, size | bbox], edge, interp) (Camera/CameraTransform.h:125-183),
+    rasterised: the image resampled from src_camera into dst_camera (both at one center, else LogicErr) through
+    reverse(p) = src.point_to_pixel(dst.pixel_to_vector(p) + C).  The output covers bbox (x0, y0, x1, y1) or a BBox2i, or
+    (0, 0, width, height) for size=(width, height); with neither, the image's own extent.  image: float32 (rows, cols) -- any
+    interpolation, zero or constant edges -- or PixelMask<float> (rows, cols, 2) {value, valid} -- bilinear, with zero,
+    constant or value edges (edge_value {value, valid}, default PixelMask<float>() = (0, 0)); numpy or CUDA.  Bit for bit the
+    reference's where both reversed coordinates are finite with |c| < 2^30; 0 ({0, 0}) elsewhere.  PointToPixelErr, naming the
+    first failing pixel, where the reference throws.  Returns a new raster where the image lives."""
+    masked = len(image.shape) == 3
+    if masked and image.shape[2] != 2 or len(image.shape) not in (2, 3):
+        raise ArgumentErr("camera_transform: the image must be float32 (rows, cols) or PixelMask<float> (rows, cols, 2)")
+    t, ptr, cols, rows, pitch, dev = _raster(image, np.float32, channels=2 if masked else 1)
+    if size is not None:
+        x0, y0, x1, y1 = 0, 0, int(size[0]), int(size[1])
+    else:
+        x0, y0, x1, y1 = _bbox(bbox) if bbox is not None else (0, 0, cols, rows)
+    ev = (C.c_float * 2)(*(edge_value if edge_value is not None else (0.0, 0.0)))
+    out = _output(t, (max(y1 - y0, 0), max(x1 - x0, 0)) + ((2,) if masked else ()), np.float32)
+    _check(lib().vwb200_camera_transform(C.byref(src_camera._struct()), C.byref(dst_camera._struct()), PIXEL_MASK_F32 if masked else PIXEL_GRAY_F32,
+                                         int(interp), int(edge), ev, ptr, cols, rows, pitch, x0, y0, _ptr(out), x1 - x0, y1 - y0, x1 - x0, dev,
+                                         _stream_ptr() if dev else None))
+    return out
+
+
+def epipolar_transformed_images(left_camera, right_camera, left_epi_camera, right_epi_camera, left_image, right_image, left_size, right_size,
+                                edge_value=(0.0, 0.0), left_roi=None, right_roi=None):
+    """epipolar_transformed_images (Camera/EpipolarUtils.cc:79-144) for PinholeModels with NULL or TSAI lenses (fitPinholeModel
+    returns those unchanged): both PixelMask<float> (rows, cols, 2) images resampled into their epipolar cameras at
+    left_size / right_size (width, height), bilinear, ValueEdgeExtension(edge_value).  A ROI whose origin is not (0, 0) (the
+    AdjustedCameraModel branch) is NoImplErr."""
+    for roi in (left_roi, right_roi):
+        if roi is not None and tuple(_bbox(roi)[:2]) != (0, 0):
+            raise NoImplErr("epipolar_transformed_images: a ROI whose origin is not (0, 0) has no device form")
+    return (camera_transform(left_image, left_camera, left_epi_camera, size=left_size, edge=EDGE_VALUE, edge_value=edge_value),
+            camera_transform(right_image, right_camera, right_epi_camera, size=right_size, edge=EDGE_VALUE, edge_value=edge_value))

@@ -225,6 +225,18 @@ template <class T> int dispmap_transform_launch(int mode, const double* m9, int 
 // disp (DispF, dw x dh, pitch dp) is read for VWB200_WARP_DISPARITY only
 int warp_launch(const vwb200_warp_params& p, const float* in, int w, int h, ptrdiff_t ip, const DispF* disp, int dw, int dh, ptrdiff_t dp,
                 int x0, int y0, float* out, int ow, int oh, ptrdiff_t op, cudaStream_t st);
+struct TriCam;
+// camera_transform (Camera/CameraTransform.h:43-183): reverse(p) = src.point_to_pixel(dst.pixel_to_vector(p) + C).  masked: the
+// pixels are PixelMask<float> {value, valid} float pairs (pitches in pairs; bilinear only, edge_value[2] for VWB200_EDGE_VALUE).
+// fail (device, 0 and ULLONG_MAX on entry): [0] is set and [1] lowered to the row-major window index of every pixel whose
+// point_to_pixel check fails.
+int camera_warp_launch(int masked, int interp, int edge, const float* edge_value, const TriCam& src, const TriCam& dst, const float* in, int w,
+                       int h, ptrdiff_t ip, int x0, int y0, float* out, int ow, int oh, ptrdiff_t op, unsigned long long* fail, cudaStream_t st);
+// compute_transformed_bbox_fast (Image/Transform.h:271-315) of the ROI (x0, y0, x1, y1) through CameraTransform(src, dst)::forward
+// into keys4 (device, fkey of min x, min y, max x, max y; the caller seeds them with BBox2f's initial bounds); fail as above,
+// with the perimeter index in the reference's loop order
+int camera_bbox_launch(const TriCam& src, const TriCam& dst, int x0, int y0, int x1, int y1, unsigned* keys4, unsigned long long* fail,
+                       cudaStream_t st);
 
 // ---- K9: fill_holes_grass over an output window (k9_inpaint.cu); T = vwb200_dispi or DispF, pitches in pixels ---------------
 // in and out are device rasters that do not overlap; stats are those of vwb200_last_fill_stats
@@ -233,8 +245,9 @@ template <class T> int fill_holes_grass_launch(const T* in, int w, int h, ptrdif
 
 // ---- K10: stereo triangulation (k10_triangulate.cu); pitches in pixels -----------------------------------------------------
 // what PinholeModel::pixel_to_vector and camera_center need, built once per call by the host: the inverse camera transform
-// (row-major), the center, the pixel pitch, the intrinsics the lens normalises by, and the Tsai parameters when tsai != 0
-struct TriCam { double inv[9], c[3], pitch, fu, fv, cu, cv, k[5]; int tsai; };
+// (row-major), the center, the pixel pitch, the intrinsics the lens normalises by, and the Tsai parameters when tsai != 0;
+// P is the 3 x 4 camera matrix K * [uvw * transpose(R) | uvw * (-transpose(R)) * C] (row-major) that point_to_pixel applies
+struct TriCam { double inv[9], c[3], pitch, fu, fv, cu, cv, k[5]; int tsai; double P[12]; };
 // stats: 5 x 8 bytes of zeroed device scratch -- [0] error sum (double), [1] max error (double bits), [2] points,
 // [3] divergent, [4] Tsai Newton-Raphson iterations; form (a) fills [4] only.  xyz pitches count {x, y, z} pixels.
 template <class T> int stereo_triangulate_launch(const T* in, ptrdiff_t ip, int x0, int y0, int ow, int oh, const TriCam& c0, const TriCam& c1,

@@ -1781,6 +1781,23 @@ static int pinhole_build(const char* what, const vwb200_pinhole& p, TriCam* c) {
   c->fu = p.fu; c->fv = p.fv; c->cu = p.cu; c->cv = p.cv;
   for (int q = 0; q < 5; ++q) c->k[q] = p.lens == VWB200_LENS_TSAI ? p.lens_params[q] : 0.0;
   c->tsai = p.lens == VWB200_LENS_TSAI;
+  // m_camera_matrix = K * [uvw * transpose(R) | (uvw * (-transpose(R))) * C], every element a dot_prod from 0.0
+  double e[12];
+  for (int i = 0; i < 3; ++i) {
+    double m2[3];
+    for (int j = 0; j < 3; ++j) {
+      e[4 * i + j] = m[3 * i + j];
+      const double nr[3] = {-p.rotation[3 * j], -p.rotation[3 * j + 1], -p.rotation[3 * j + 2]};
+      m2[j] = dot3h(uvw[i], nr);
+    }
+    e[4 * i + 3] = dot3h(m2, p.center);
+  }
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 4; ++j) {
+      double r = 0.0;
+      for (int q = 0; q < 3; ++q) r += k[3 * i + q] * e[4 * q + j];
+      c->P[4 * i + j] = r;
+    }
   return VWB200_OK;
 }
 
@@ -1909,6 +1926,248 @@ int vwb200_universe_radius(const double* in, int w, int h, ptrdiff_t pitch, cons
   VWB_TRY(c.finish());
   if (rejected) *rejected = (long long)s[0];
   if (total) *total = (long long)w * h;
+  return VWB200_OK;
+}
+
+// ---- epipolar rectification (Camera/PinholeModel.cc:679-732, EpipolarUtils.cc:37-76, CameraTransform.h) -----------------------
+static void cross3h(const double* a, const double* b, double* r) {
+  r[0] = a[1] * b[2] - a[2] * b[1];
+  r[1] = a[2] * b[0] - a[0] * b[2];
+  r[2] = a[0] * b[1] - a[1] * b[0];
+}
+
+// camera_pose().rotation_matrix(): Quaternion(R) (Math/Quaternion.h:211-252), branching on the largest of ww, xx, yy, zz, then
+// rotation_matrix() (:314-335)
+static void quaternion_round_trip(const double* R, double* out) {
+  const double d0 = R[0], d1 = R[4], d2 = R[8];
+  const double ww = 1.0 + d0 + d1 + d2, xx = 1.0 + d0 - d1 - d2, yy = 1.0 - d0 + d1 - d2, zz = 1.0 - d0 - d1 + d2;
+  double mx = ww;
+  if (xx > mx) mx = xx;
+  if (yy > mx) mx = yy;
+  if (zz > mx) mx = zz;
+  double q[4];
+  if (ww == mx) {
+    const double w4 = std::sqrt(ww * 4.0);
+    q[0] = w4 / 4; q[1] = (R[7] - R[5]) / w4; q[2] = (R[2] - R[6]) / w4; q[3] = (R[3] - R[1]) / w4;
+  } else if (xx == mx) {
+    const double x4 = std::sqrt(xx * 4.0);
+    q[0] = (R[7] - R[5]) / x4; q[1] = x4 / 4; q[2] = (R[1] + R[3]) / x4; q[3] = (R[2] + R[6]) / x4;
+  } else if (yy == mx) {
+    const double y4 = std::sqrt(yy * 4.0);
+    q[0] = (R[2] - R[6]) / y4; q[1] = (R[1] + R[3]) / y4; q[2] = y4 / 4; q[3] = (R[5] + R[7]) / y4;
+  } else {
+    const double z4 = std::sqrt(zz * 4.0);
+    q[0] = (R[3] - R[1]) / z4; q[1] = (R[2] + R[6]) / z4; q[2] = (R[5] + R[7]) / z4; q[3] = z4 / 4;
+  }
+  const double w = q[0], x = q[1], y = q[2], z = q[3];
+  const double w2 = w * w, x2 = x * x, y2 = y * y, z2 = z * z, wx = w * x, wy = w * y, wz = w * z, xy = x * y, yz = y * z, zx = z * x;
+  out[0] = w2 + x2 - y2 - z2; out[4] = w2 - x2 + y2 - z2; out[8] = w2 - x2 - y2 + z2;
+  out[1] = 2 * (xy - wz); out[2] = 2 * (zx + wy); out[5] = 2 * (yz - wx);
+  out[3] = 2 * (xy + wz); out[6] = 2 * (zx - wy); out[7] = 2 * (yz + wx);
+}
+
+int vwb200_pinhole_epipolar(const vwb200_pinhole* cam0, const vwb200_pinhole* cam1, vwb200_pinhole* epi0, vwb200_pinhole* epi1) {
+  const char* what = "epipolar";
+  if (!epi0 || !epi1) { set_error("%s: null output camera", what); return VWB200_EARG; }
+  VWB_TRY(pinhole_check(what, cam0));
+  VWB_TRY(pinhole_check(what, cam1));
+  TriCam t;
+  VWB_TRY(pinhole_build(what, *cam0, &t));                  // the source cameras must be ones the reference can construct
+  VWB_TRY(pinhole_build(what, *cam1, &t));
+  double rot0[9], rot1[9];
+  quaternion_round_trip(cam0->rotation, rot0);
+  quaternion_round_trip(cam1->rotation, rot1);
+  const double look0[3] = {-1 * rot0[2], -1 * rot0[5], -1 * rot0[8]}, look1[3] = {-1 * rot1[2], -1 * rot1[5], -1 * rot1[8]};
+  double d[3], u[3], mean[3], t1[3], tmp[3], w[3], v[3];
+  for (int i = 0; i < 3; ++i) d[i] = cam1->center[i] - cam0->center[i];
+  const double nd = std::sqrt(dot3h(d, d));
+  for (int i = 0; i < 3; ++i) { u[i] = d[i] / nd; mean[i] = (look0[i] + look1[i]) / 2.0; }
+  cross3h(mean, u, t1);
+  cross3h(u, t1, tmp);
+  const double nt = std::sqrt(dot3h(tmp, tmp));
+  for (int i = 0; i < 3; ++i) w[i] = tmp[i] / nt;
+  cross3h(w, u, v);
+  vwb200_pinhole e{};
+  for (int i = 0; i < 3; ++i) { e.rotation[3 * i] = u[i]; e.rotation[3 * i + 1] = -v[i]; e.rotation[3 * i + 2] = -w[i]; }
+  e.fu = (cam0->fu + cam1->fu) / 2.0; e.fv = (cam0->fv + cam1->fv) / 2.0;
+  e.cu = (cam0->cu + cam1->cu) / 2.0; e.cv = (cam0->cv + cam1->cv) / 2.0;
+  e.pixel_pitch = (cam0->pixel_pitch + cam1->pixel_pitch) / 2.0;
+  e.u_direction[0] = e.v_direction[1] = e.w_direction[2] = 1.0;
+  e.lens = VWB200_LENS_NULL;
+  vwb200_pinhole e1 = e;                                    // the outputs may be the inputs
+  std::memcpy(e.center, cam0->center, sizeof e.center);
+  std::memcpy(e1.center, cam1->center, sizeof e.center);
+  *epi0 = e;
+  *epi1 = e1;
+  return VWB200_OK;
+}
+
+struct MaskF { float v, valid; };                                // PixelMask<float>
+
+// CameraTransform's VW_ASSERT (CameraTransform.h:53, 66): both cameras at one center
+static int same_center(const char* what, const TriCam& a, const TriCam& b) {
+  if (a.c[0] == b.c[0] && a.c[1] == b.c[1] && a.c[2] == b.c[2]) return VWB200_OK;
+  set_error("%s: CameraTransformFunctor: Camera transformation require that the camera center is always the same for both cameras.", what);
+  return VWB200_ELOGIC;
+}
+
+static int projection_error(const char* what, long long x, long long y) {
+  set_error("%s: PinholeModel: Projection into pinhole camera is inaccurate. (first failing pixel (%lld, %lld))", what, x, y);
+  return VWB200_EPROJECT;
+}
+
+// the perimeter index k of compute_transformed_bbox_fast over (x0, y0, x1, y1) as a pixel
+static void perimeter_pixel(const int32_t* r, long long k, long long* x, long long* y) {
+  const long long cw = (long long)r[2] - r[0], ch = (long long)r[3] - r[1];
+  if (k < cw) { *x = r[0] + k; *y = r[1]; }
+  else if (k < 2 * cw) { *x = r[0] + k - cw; *y = r[3] - 1LL; }
+  else if (k < 2 * cw + ch) { *x = r[0]; *y = r[1] + k - 2 * cw; }
+  else { *x = r[2] - 1LL; *y = r[1] + k - 2 * cw - ch; }
+}
+
+static float key_float(unsigned k) {                           // kfloat on the host
+  const unsigned u = (k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k;
+  float f;
+  std::memcpy(&f, &u, sizeof f);
+  return f;
+}
+static unsigned float_key(float f) {
+  unsigned u;
+  std::memcpy(&u, &f, sizeof u);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+// both cameras' compute_transformed_bbox_fast through CameraTransform(cam, epi)::forward: bbox[cam] = {min x, min y, max x, max y}
+static int epipolar_bboxes(AbiCall& c, const TriCam* cam, const TriCam* epi, const int32_t* const* roi, float (*bbox)[4]) {
+  unsigned* keys;
+  unsigned long long* fail;
+  VWB_TRY(c.ar.alloc(&keys, 8));
+  VWB_TRY(c.ar.alloc(&fail, 4));
+  const float big = (float)(INT32_MAX - 1);                    // BBox2f's initial bounds (Math/BBox.tcc:38-45)
+  const unsigned init[8] = {float_key(big), float_key(big), float_key(-big), float_key(-big),
+                            float_key(big), float_key(big), float_key(-big), float_key(-big)};
+  const unsigned long long finit[4] = {0, ULLONG_MAX, 0, ULLONG_MAX};
+  VWB_CUDA(cudaMemcpyAsync(keys, init, sizeof init, cudaMemcpyHostToDevice, c.st));
+  VWB_CUDA(cudaMemcpyAsync(fail, finit, sizeof finit, cudaMemcpyHostToDevice, c.st));
+  for (int i = 0; i < 2; ++i)
+    VWB_TRY(camera_bbox_launch(cam[i], epi[i], roi[i][0], roi[i][1], roi[i][2], roi[i][3], keys + 4 * i, fail + 2 * i, c.st));
+  unsigned k[8];
+  unsigned long long f[4];
+  VWB_CUDA(cudaMemcpyAsync(k, keys, sizeof k, cudaMemcpyDeviceToHost, c.st));
+  VWB_CUDA(cudaMemcpyAsync(f, fail, sizeof f, cudaMemcpyDeviceToHost, c.st));
+  VWB_CUDA(cudaStreamSynchronize(c.st));
+  for (int i = 0; i < 2; ++i)
+    if (f[2 * i]) {                                            // the reference throws at the first failing point of the first camera
+      long long x, y;
+      perimeter_pixel(roi[i], (long long)f[2 * i + 1], &x, &y);
+      return projection_error("resize_epipolar_cameras_to_fit", x, y);
+    }
+  for (int i = 0; i < 8; ++i) bbox[i / 4][i % 4] = key_float(k[i]);
+  return VWB200_OK;
+}
+
+static int roi_check(const char* what, const int32_t* r) {
+  if (!r) { set_error("%s: null ROI", what); return VWB200_EARG; }
+  if (r[2] < r[0] || r[3] < r[1]) { set_error("%s: bad ROI (%d, %d, %d, %d)", what, r[0], r[1], r[2], r[3]); return VWB200_EARG; }
+  return VWB200_OK;
+}
+
+int vwb200_resize_epipolar_cameras_to_fit(const vwb200_pinhole* cam1, const vwb200_pinhole* cam2, vwb200_pinhole* epi1, vwb200_pinhole* epi2,
+                                          const int32_t roi1[4], const int32_t roi2[4], int32_t size1[2], int32_t size2[2], void* stream) {
+  const char* what = "resize_epipolar_cameras_to_fit";
+  if (!size1 || !size2) { set_error("%s: null output size", what); return VWB200_EARG; }
+  VWB_TRY(pinhole_check(what, cam1));
+  VWB_TRY(pinhole_check(what, cam2));
+  VWB_TRY(pinhole_check(what, epi1));
+  VWB_TRY(pinhole_check(what, epi2));
+  VWB_TRY(roi_check(what, roi1));
+  VWB_TRY(roi_check(what, roi2));
+  TriCam cam[2], epi[2];
+  VWB_TRY(pinhole_build(what, *cam1, &cam[0]));
+  VWB_TRY(pinhole_build(what, *cam2, &cam[1]));
+  VWB_TRY(pinhole_build(what, *epi1, &epi[0]));
+  VWB_TRY(pinhole_build(what, *epi2, &epi[1]));
+  VWB_TRY(same_center(what, cam[0], epi[0]));
+  VWB_TRY(same_center(what, cam[1], epi[1]));
+  VWB_TRY(ensure_device());
+  AbiCall c;
+  VWB_TRY(c.open(stream, 0));
+  const int32_t* roi[2] = {roi1, roi2};
+  float bb[2][4];
+  VWB_TRY(epipolar_bboxes(c, cam, epi, roi, bb));
+  // shift both principal points by the leftmost / uppermost corner (in CCD units), from epi1's offset (EpipolarUtils.cc:52-65)
+  const double min_col = std::min(bb[0][0], bb[1][0]), min_row = std::min(bb[0][1], bb[1][1]);
+  const double cu = epi1->cu - min_col * epi1->pixel_pitch, cv = epi1->cv - min_row * epi1->pixel_pitch;
+  vwb200_pinhole e1 = *epi1, e2 = *epi2;
+  e1.cu = e2.cu = cu;
+  e1.cv = e2.cv = cv;
+  VWB_TRY(pinhole_build(what, e1, &epi[0]));
+  VWB_TRY(pinhole_build(what, e2, &epi[1]));
+  VWB_TRY(epipolar_bboxes(c, cam, epi, roi, bb));
+  VWB_TRY(c.finish());
+  *epi1 = e1;
+  *epi2 = e2;
+  size1[0] = (int32_t)bb[0][2]; size1[1] = (int32_t)bb[0][3];    // Vector2i(bbox.max()): truncation toward zero
+  size2[0] = (int32_t)bb[1][2]; size2[1] = (int32_t)bb[1][3];
+  return VWB200_OK;
+}
+
+int vwb200_camera_transform(const vwb200_pinhole* src, const vwb200_pinhole* dst, int pixel_type, int interp, int edge, const float edge_value[2],
+                            const void* in, int w, int h, ptrdiff_t pitch, int x0, int y0, void* out, int ow, int oh, ptrdiff_t opitch,
+                            int on_device, void* stream) {
+  const char* what = "camera_transform";
+  if (!in || !out) { set_error("%s: null input or output", what); return VWB200_EARG; }
+  VWB_TRY(pinhole_check(what, src));
+  VWB_TRY(pinhole_check(what, dst));
+  if (pixel_type != VWB200_PIXEL_GRAY_F32 && pixel_type != VWB200_PIXEL_MASK_F32) { set_error("%s: unknown pixel type %d", what, pixel_type); return VWB200_EARG; }
+  if (interp != VWB200_INTERP_BILINEAR && interp != VWB200_INTERP_BICUBIC && interp != VWB200_INTERP_NEAREST) {
+    set_error("%s: unknown interpolation %d", what, interp);
+    return VWB200_EARG;
+  }
+  if (edge != VWB200_EDGE_ZERO && edge != VWB200_EDGE_CONSTANT && edge != VWB200_EDGE_VALUE) { set_error("%s: unknown edge extension %d", what, edge); return VWB200_EARG; }
+  if (w <= 0 || h <= 0 || pitch < w) { set_error("%s: bad image size %d x %d, pitch %td", what, w, h, pitch); return VWB200_EARG; }
+  if (ow <= 0 || oh <= 0 || opitch < ow) { set_error("%s: bad output size %d x %d, pitch %td", what, ow, oh, opitch); return VWB200_EARG; }
+  if ((long long)x0 + ow - 1 > INT_MAX || (long long)y0 + oh - 1 > INT_MAX) {
+    set_error("%s: the window (%d, %d, %d, %d) leaves the int32 pixel coordinates", what, x0, y0, ow, oh);
+    return VWB200_EARG;
+  }
+  const bool masked = pixel_type == VWB200_PIXEL_MASK_F32;
+  const size_t px = masked ? 8 : 4;
+  if (rasters_overlap(in, w, h, pitch, out, ow, oh, opitch, px, px)) { set_error("%s: out overlaps the image", what); return VWB200_EARG; }
+  if (edge == VWB200_EDGE_VALUE && !edge_value) { set_error("%s: ValueEdgeExtension needs an edge value", what); return VWB200_EARG; }
+  if ((masked && interp != VWB200_INTERP_BILINEAR) || (!masked && edge == VWB200_EDGE_VALUE)) {
+    set_error("%s: %s has no device form (PixelMask<float> takes bilinear interpolation, ValueEdgeExtension PixelMask<float> pixels)", what,
+              masked ? "this interpolation of PixelMask<float> pixels" : "ValueEdgeExtension of float pixels");
+    return VWB200_ENOIMPL;
+  }
+  const float ev[2] = {edge_value ? edge_value[0] : 0.0f, edge_value ? edge_value[1] : 0.0f};
+  TriCam s, d;
+  VWB_TRY(pinhole_build(what, *src, &s));
+  VWB_TRY(pinhole_build(what, *dst, &d));
+  VWB_TRY(same_center(what, s, d));
+  VWB_TRY(ensure_device());
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
+  const float* din; ptrdiff_t dp;
+  float* dout; ptrdiff_t dop;
+  if (masked) {                                                  // {value, valid} pairs, staged as such
+    const MaskF* mi; MaskF* mo;
+    VWB_TRY(c.in((const MaskF*)in, w, h, pitch, on_device, &mi, &dp));
+    VWB_TRY(c.out((MaskF*)out, ow, oh, opitch, on_device, &mo, &dop));
+    din = (const float*)mi; dout = (float*)mo;
+  } else {
+    VWB_TRY(c.in((const float*)in, w, h, pitch, on_device, &din, &dp));
+    VWB_TRY(c.out((float*)out, ow, oh, opitch, on_device, &dout, &dop));
+  }
+  unsigned long long* fail;
+  VWB_TRY(c.ar.alloc(&fail, 2));
+  const unsigned long long finit[2] = {0, ULLONG_MAX};
+  VWB_CUDA(cudaMemcpyAsync(fail, finit, sizeof finit, cudaMemcpyHostToDevice, c.st));
+  VWB_TRY(camera_warp_launch(masked, interp, edge, ev, s, d, din, w, h, dp, x0, y0, dout, ow, oh, dop, fail, c.st));
+  unsigned long long f[2];
+  VWB_CUDA(cudaMemcpyAsync(f, fail, sizeof f, cudaMemcpyDeviceToHost, c.st));
+  VWB_TRY(c.finish());
+  if (f[0]) return projection_error(what, x0 + (long long)(f[1] % (unsigned long long)ow), y0 + (long long)(f[1] / (unsigned long long)ow));
   return VWB200_OK;
 }
 

@@ -5,7 +5,11 @@
 // Transform() has a zero tolerance, so TransformView::rasterize never builds an ApproximateTransform grid: every output pixel
 // is a function of its own coordinates.  Each step is an explicitly rounded intrinsic in the reference's order (no
 // contraction), so the results are bit for bit those of the reference built with -ffp-contract=off.
-#include "common.cuh"
+// The internal kinds kCamera (float pixels) and kCameraMasked (PixelMask<float>, bilinear) are CameraTransform(src, dst)
+// (Camera/CameraTransform.h:52-61) between pinhole cameras, through pinhole.cuh: reverse(p) = src.point_to_pixel(
+// dst.pixel_to_vector(p) + C), with point_to_pixel's check.  k8_camera_bbox_kernel is the bbox pass of
+// resize_epipolar_cameras_to_fit through the same cameras.
+#include "pinhole.cuh"
 
 namespace vwb200 {
 namespace {
@@ -14,6 +18,8 @@ constexpr int kMaxGridY = 65535;                       // the row tiles of talle
 constexpr int kTW = 32, kTH = 8;
 // the reversed coordinates the contract covers: beyond them the reference converts out of int32 range (undefined)
 constexpr double kDomain = 1073741824.0;               // 2^30
+constexpr int kCamera = 2;                             // beside VWB200_WARP_HOMOGRAPHY and VWB200_WARP_DISPARITY
+constexpr int kCameraMasked = 3;                       // kCamera over PixelMask<float> {value, valid} pixels
 
 // math::impl::_floor and _round for double -> int32 (Math/Functions.h:48-51, 74-81)
 __device__ __forceinline__ int vw_floor(double v) {
@@ -51,6 +57,46 @@ __device__ __forceinline__ float bilinear(const float* __restrict__ in, int w, i
   return __fadd_rn(r, __fmul_rn(row, ny));
 }
 
+// PixelMask<float> {value, valid} pixels (pitches in pixels).  Zero extension is PixelMask<float>() = {0, 0} (Image/PixelMask.h:59-62),
+// value extension the edge pixel as given (Image/EdgeExtension.h:66-76)
+struct Px2 { float v, valid; };
+template <int Edge>
+__device__ __forceinline__ Px2 pixel2(const float* __restrict__ in, int w, int h, ptrdiff_t ip, float2 ev, int i, int j) {
+  if (Edge != VWB200_EDGE_CONSTANT) {
+    if (i >= 0 && j >= 0 && i < w && j < h) {
+      const float* q = in + 2 * ((ptrdiff_t)j * ip + i);
+      return Px2{__ldg(q), __ldg(q + 1)};
+    }
+    return Edge == VWB200_EDGE_ZERO ? Px2{0.0f, 0.0f} : Px2{ev.x, ev.y};
+  }
+  i = i < 0 ? 0 : (i >= w ? w - 1 : i);
+  j = j < 0 ? 0 : (j >= h ? h - 1 : j);
+  const float* q = in + 2 * ((ptrdiff_t)j * ip + i);
+  return Px2{__ldg(q), __ldg(q + 1)};
+}
+// BilinearInterpolationImpl on PixelMask<float> (Image/PixelMask.h:321-380, 499-626): pixel * scalar and channel_cast give
+// valid = (valid != 0) as 1.0f / 0.0f (NaN counts as valid), += ANDs the validity, *= scalar keeps it.  So the integral
+// shortcut returns {value, valid != 0}, and the interpolated value is the float one's with valid = all four neighbours' valid != 0.
+template <int Edge>
+__device__ __forceinline__ Px2 bilinear2(const float* __restrict__ in, int w, int h, ptrdiff_t ip, float2 ev, double i, double j) {
+  const int x = vw_floor(i), y = vw_floor(j);
+  if ((double)x == i && (double)y == j) {
+    const Px2 p = pixel2<Edge>(in, w, h, ip, ev, x, y);
+    return Px2{p.v, p.valid != 0.0f ? 1.0f : 0.0f};
+  }
+  const float nx = __fsub_rn(__double2float_rn(i), __int2float_rn(x)), ny = __fsub_rn(__double2float_rn(j), __int2float_rn(y));
+  const float n1mx = __fsub_rn(1.0f, nx), n1my = __fsub_rn(1.0f, ny);
+  const Px2 p00 = pixel2<Edge>(in, w, h, ip, ev, x, y), p10 = pixel2<Edge>(in, w, h, ip, ev, x + 1, y);
+  const Px2 p01 = pixel2<Edge>(in, w, h, ip, ev, x, y + 1), p11 = pixel2<Edge>(in, w, h, ip, ev, x + 1, y + 1);
+  float r = __fmul_rn(p00.v, n1mx);
+  r = __fadd_rn(r, __fmul_rn(p10.v, nx));
+  r = __fmul_rn(r, n1my);
+  float row = __fmul_rn(p01.v, n1mx);
+  row = __fadd_rn(row, __fmul_rn(p11.v, nx));
+  const bool ok = p00.valid != 0.0f && p10.valid != 0.0f && p01.valid != 0.0f && p11.valid != 0.0f;
+  return Px2{__fadd_rn(r, __fmul_rn(row, ny)), ok ? 1.0f : 0.0f};
+}
+
 // BicubicInterpolationImpl (:138-186) in double
 __device__ __forceinline__ void cubic_weights(double n, double& w0, double& w1, double& w2, double& w3) {
   w0 = __dmul_rn(__dsub_rn(__dmul_rn(__dsub_rn(2.0, n), n), 1.0), n);                      // ((2-n)*n-1)*n
@@ -85,6 +131,9 @@ struct WarpArgs {
   double m[9];
   int x0, y0;
   float* out; int ow, oh; ptrdiff_t op;
+  TriCam src, dst;                                     // kCamera only (appended: the other kinds' parameters keep their offsets)
+  unsigned long long* fail;                            // kCamera: {any check failed, first failing row-major window index}
+  float2 ev;                                           // kCameraMasked: the VWB200_EDGE_VALUE pixel {value, valid}
 };
 
 // one thread per output pixel of a 32 x 8 tile; window pixel (ox, oy) is TransformView pixel (x0 + ox, y0 + oy)
@@ -102,6 +151,14 @@ __global__ void __launch_bounds__(kTW * kTH) k8_warp_kernel(const WarpArgs a) {
       const double w = __dadd_rn(__dadd_rn(__dmul_rn(a.m[6], px), __dmul_rn(a.m[7], py)), a.m[8]);
       rx = __ddiv_rn(__dadd_rn(__dadd_rn(__dmul_rn(a.m[0], px), __dmul_rn(a.m[1], py)), a.m[2]), w);
       ry = __ddiv_rn(__dadd_rn(__dadd_rn(__dmul_rn(a.m[3], px), __dmul_rn(a.m[4], py)), a.m[5]), w);
+    } else if (Kind == kCamera || Kind == kCameraMasked) {
+      bool ok;
+      int iters = 0;
+      camera_map<true>(a.dst, a.src, px, py, &rx, &ry, &ok, &iters);
+      if (!ok) {                                       // the reference throws PointToPixelErr: flag it, keep the first pixel
+        a.fail[0] = 1;
+        atomicMin(a.fail + 1, (unsigned long long)oy * a.ow + ox);
+      }
     } else {
       // DisparityTransform::reverse: the offset read with nearest-pixel interpolation and zero extension at the integer p
       const int ix = a.x0 + ox;
@@ -110,6 +167,14 @@ __global__ void __launch_bounds__(kTW * kTH) k8_warp_kernel(const WarpArgs a) {
         const float* d = reinterpret_cast<const float*>(a.disp + (ptrdiff_t)iy * a.dp + ix);
         if (__ldg(d + 2) != 0.0f) { rx = __dadd_rn(px, (double)__ldg(d)); ry = __dadd_rn(py, (double)__ldg(d + 1)); }
       }
+    }
+    if (Kind == kCameraMasked) {
+      Px2 v{0.0f, 0.0f};                               // outside the domain: {0, 0}
+      if (fabs(rx) < kDomain && fabs(ry) < kDomain) v = bilinear2<Edge>(a.in, a.w, a.h, a.ip, a.ev, rx, ry);
+      float* q = a.out + 2 * ((ptrdiff_t)oy * a.op + ox);
+      q[0] = v.v;
+      q[1] = v.valid;
+      continue;
     }
     float v = 0.0f;                                    // outside the domain (and NaN / inf): 0.0f
     if (fabs(rx) < kDomain && fabs(ry) < kDomain) {
@@ -139,12 +204,53 @@ int launch_interp(int interp, int edge, const WarpArgs& a, cudaStream_t st) {
   return launch_edge<Kind, VWB200_INTERP_NEAREST>(edge, a, st);
 }
 
+// perimeter point k of compute_transformed_bbox_fast's four loops (top, bottom, left, right edges) through forward(), grown
+// into a BBox2f: NaN coordinates compare false and are skipped, the others enter as float(c), so the bounds are the float
+// order statistics whatever the order (a bound that rounds to zero may carry the other sign of zero)
+__global__ void __launch_bounds__(128) k8_camera_bbox_kernel(const TriCam src, const TriCam dst, int x0, int y0, int x1, int y1,
+                                                             unsigned* keys, unsigned long long* fail) {
+  const long long cw = (long long)x1 - x0, ch = (long long)y1 - y0;
+  const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= 2 * (cw + ch)) return;
+  double px, py;
+  if (k < cw) { px = (double)(x0 + k); py = (double)y0; }
+  else if (k < 2 * cw) { px = (double)(x0 + (k - cw)); py = (double)(y1 - 1); }
+  else if (k < 2 * cw + ch) { px = (double)x0; py = (double)(y0 + (k - 2 * cw)); }
+  else { px = (double)(x1 - 1); py = (double)(y0 + (k - 2 * cw - ch)); }
+  double u, v;
+  bool ok;
+  int iters = 0;
+  camera_map<true>(src, dst, px, py, &u, &v, &ok, &iters);
+  if (!ok) { fail[0] = 1; atomicMin(fail + 1, (unsigned long long)k); return; }
+  if (u == u) { atomicMin(keys, fkey(__double2float_rn(u))); atomicMax(keys + 2, fkey(__double2float_rn(u))); }
+  if (v == v) { atomicMin(keys + 1, fkey(__double2float_rn(v))); atomicMax(keys + 3, fkey(__double2float_rn(v))); }
+}
+
 }  // namespace
+
+int camera_warp_launch(int masked, int interp, int edge, const float* edge_value, const TriCam& src, const TriCam& dst, const float* in, int w,
+                       int h, ptrdiff_t ip, int x0, int y0, float* out, int ow, int oh, ptrdiff_t op, unsigned long long* fail, cudaStream_t st) {
+  if (ow <= 0 || oh <= 0) return VWB200_OK;
+  WarpArgs a{in, w, h, ip, nullptr, 0, 0, 0, {}, x0, y0, out, ow, oh, op, src, dst, fail, make_float2(edge_value[0], edge_value[1])};
+  if (!masked) return launch_interp<kCamera>(interp, edge, a, st);
+  if (edge == VWB200_EDGE_ZERO) return launch<kCameraMasked, VWB200_INTERP_BILINEAR, VWB200_EDGE_ZERO>(a, st);
+  if (edge == VWB200_EDGE_CONSTANT) return launch<kCameraMasked, VWB200_INTERP_BILINEAR, VWB200_EDGE_CONSTANT>(a, st);
+  return launch<kCameraMasked, VWB200_INTERP_BILINEAR, VWB200_EDGE_VALUE>(a, st);
+}
+
+int camera_bbox_launch(const TriCam& src, const TriCam& dst, int x0, int y0, int x1, int y1, unsigned* keys4, unsigned long long* fail,
+                       cudaStream_t st) {
+  const long long n = 2 * ((long long)x1 - x0 + (long long)y1 - y0);
+  if (n <= 0) return VWB200_OK;
+  k8_camera_bbox_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(src, dst, x0, y0, x1, y1, keys4, fail);
+  VWB_LAUNCH_CHECK();
+  return VWB200_OK;
+}
 
 int warp_launch(const vwb200_warp_params& p, const float* in, int w, int h, ptrdiff_t ip, const DispF* disp, int dw, int dh, ptrdiff_t dp,
                 int x0, int y0, float* out, int ow, int oh, ptrdiff_t op, cudaStream_t st) {
   if (ow <= 0 || oh <= 0) return VWB200_OK;
-  WarpArgs a{in, w, h, ip, disp, dw, dh, dp, {}, x0, y0, out, ow, oh, op};
+  WarpArgs a{in, w, h, ip, disp, dw, dh, dp, {}, x0, y0, out, ow, oh, op, {}, {}, nullptr, {}};
   for (int i = 0; i < 9; ++i) a.m[i] = p.matrix[i];
   if (p.kind == VWB200_WARP_HOMOGRAPHY) return launch_interp<VWB200_WARP_HOMOGRAPHY>(p.interp, p.edge, a, st);
   return launch_interp<VWB200_WARP_DISPARITY>(p.interp, p.edge, a, st);
