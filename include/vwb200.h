@@ -328,6 +328,37 @@ int vwb200_camera_transform(const vwb200_pinhole* src, const vwb200_pinhole* dst
                             int on_device, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Exact interest point matching: InterestPointMatcherSimple<L2NormMetric | HammingMetric, NullConstraint>::operator()
+ * (src/vw/InterestPoint/Matcher.h:415-509, Matcher.cc:33-100) and remove_duplicates (Matcher.cc:151-195).
+ * desc1 is n1 x dim floats (row pitch pitch1 floats), desc2 n2 x dim (pitch2); pol1 / pol2 hold one polarity byte per point
+ * (compared as bools).  For each query i the candidates j = 0..n2-1 of equal polarity are scanned; the distance is the
+ * reference's float metric:
+ *   VWB200_METRIC_L2       sum over k in order of (a - b) * (a - b), each sub, mul and add rounded to float (no FMA);
+ *   VWB200_METRIC_HAMMING  the popcount of the XOR of the bytes static_cast<uint8>(value) (truncation), exact for 8 dim <= 2^24
+ *                          (larger dim: VWB200_ENOIMPL).  A value outside (-1, 256) or NaN, undefined in the reference, is
+ *                          VWB200_EARG naming the first such element.
+ * first / second are the reference's double first_pick / second_pick (1e100 when none: an inf or NaN distance is never
+ * picked; among equal minima the lowest j wins; a distance equal to first becomes second), and match_index[i] is the picked
+ * j, or -1 when none was picked or first > threshold * second in double (threshold may be any double).  n2 == 0 gives -1
+ * everywhere (the reference's empty-list early return).  match_index is int32; first / second may be NULL.  Exactness: every
+ * index and double bit for bit the reference's.  VWB200_EARG, before the device is looked up, for a NULL pointer with n > 0,
+ * n1, n2, dim < 0, a pitch below dim, an unknown metric, and outputs that overlap each other or an input.
+ * ------------------------------------------------------------------------------------------- */
+enum { VWB200_METRIC_L2 = 0, VWB200_METRIC_HAMMING = 1 };
+int vwb200_ip_match(int metric, const float* desc1, const uint8_t* pol1, int n1, const float* desc2, const uint8_t* pol2, int n2,
+                    int dim, ptrdiff_t pitch1, ptrdiff_t pitch2, double threshold, int32_t* match_index, double* first, double* second,
+                    int on_device, void* stream);
+/* the last vwb200_ip_match on this thread: descriptor pairs scanned (n1 * n2), the metric, the CTAs the candidate range was
+ * split over (1: not split; 0: no candidates) and the matches kept */
+typedef struct { long long pairs, matches; int32_t metric, splits; } vwb200_ipmatch_stats;
+int vwb200_last_ipmatch_stats(vwb200_ipmatch_stats* out);
+/* remove_duplicates on the host: pairs are walked from last to first; a pair is dropped when its (x1, y1) or its (x2, y2) was
+ * already kept (compared as std::pair<float, float>, so -0.0 equals 0.0), and kept otherwise.  xy1 / xy2 hold n (x, y)
+ * float pairs; keep receives the kept indices in ascending order, *n_kept their count.  A NaN coordinate, which breaks the
+ * reference's std::set ordering, is VWB200_EARG. */
+int vwb200_remove_duplicate_matches(const float* xy1, const float* xy2, int n, int32_t* keep, int* n_kept);
+
+/* ---------------------------------------------------------------------------------------------
  * vw::stereo::ParabolaSubpixelView::rasterize(dest, bbox) (src/vw/Stereo/ParabolaSubpixelView.h:27-117,
  * .cc:31-330): 3x3 AbsoluteCost patch around the integer disparity, 6x9 pseudo-inverse parabola fit,
  * offset kept when its norm is below 5.  disparity: cols x rows PixelMask<Vector2f> triples (same size as

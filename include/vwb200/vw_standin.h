@@ -18,6 +18,9 @@
 //   camera::CameraModel, PinholeModel, NullLensDistortion, TsaiLensDistortion
 //                               Camera/CameraModel.h, PinholeModel.h:158-261, LensDistortion.h (constructors and accessors only)
 //   camera::PointToPixelErr     Camera/CameraModel.h:229
+//   ip::InterestPoint           InterestPoint/InterestPoint.h:45-110 (fields and constructor; descriptor as std::vector<float>)
+//   ip::L2NormMetric, HammingMetric, NullConstraint   InterestPoint/Matcher.h (tag types only)
+//   ProgressCallback            Core/ProgressCallback.h (dummy_instance() and the calls the matchers make)
 #pragma once
 #include <vector>
 #include <cstddef>
@@ -282,6 +285,38 @@ public:
   LensDistortion const* lens_distortion() const { return m_distortion.get(); }
 };
 }  // namespace camera
+
+class ProgressCallback {                                                                      // Core/ProgressCallback.h
+public:
+  virtual ~ProgressCallback() {}
+  static ProgressCallback const& dummy_instance() { static ProgressCallback d; return d; }
+  virtual void report_progress(double) const {}
+  virtual void report_incremental_progress(double) const {}
+  virtual void report_finished() const {}
+  virtual bool abort_requested() const { return false; }
+};
+
+namespace ip {
+struct InterestPoint {                                                                        // InterestPoint/InterestPoint.h:45-110
+  typedef std::vector<float> descriptor_type;
+  InterestPoint(float x = 0, float y = 0, float scale = 1.0, float interest = 0.0, float ori = 0.0, bool pol = false, uint32_t octave = 0,
+                uint32_t scale_lvl = 0)
+    : x(x), y(y), scale(scale), ix(int32(x)), iy(int32(y)), orientation(ori), interest(interest), polarity(pol), octave(octave),
+      scale_lvl(scale_lvl) {}
+  float x, y;
+  float scale;
+  int32 ix, iy;
+  float orientation;
+  float interest;
+  bool polarity;
+  uint32_t octave, scale_lvl;
+  descriptor_type descriptor;
+  size_t size() const { return descriptor.size(); }
+};
+struct L2NormMetric {};
+struct HammingMetric {};
+struct NullConstraint {};
+}  // namespace ip
 
 namespace stereo {
 struct SemiGlobalMatcher {                                                                    // Stereo/SGM.h:93-99

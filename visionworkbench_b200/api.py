@@ -23,6 +23,9 @@ Names, argument order and error behaviour follow Vision Workbench:
     universe_radius           -- src/vw/Camera/PinholeModel.cc:79-116, Stereo/StereoView.h:74-186, StereoModel.cc:254-309
   * epipolar, resize_epipolar_cameras_to_fit, camera_transform, epipolar_transformed_images (float32 or PixelMask<float>
     images)                   -- src/vw/Camera/PinholeModel.cc:351-397, 679-732, EpipolarUtils.cc:37-144, CameraTransform.h
+  * ip_match (InterestPointMatcherSimple, L2 or Hamming), remove_duplicates, read/write_binary_ip_file,
+    read/write_binary_match_file
+                              -- src/vw/InterestPoint/Matcher.h:415-509, Matcher.cc:33-195, MatcherIO.cc:248-366
 
 There is no CPU path: every call goes to libvwb200.so (hand-written sm_90a kernels) and raises if
 the library or a CUDA device is missing.  Inputs may be numpy arrays (staged through HBM by the
@@ -153,6 +156,9 @@ def lib():
         L.vwb200_pinhole_epipolar.argtypes = [PH, PH, PH, PH]
         L.vwb200_resize_epipolar_cameras_to_fit.argtypes = [PH, PH, PH, PH, P, P, P, P, P]
         L.vwb200_camera_transform.argtypes = [PH, PH, I, I, I, P, P, I, I, Z, I, I, P, I, I, Z, I, P]
+        L.vwb200_ip_match.argtypes = [I, P, P, I, P, P, I, I, Z, Z, D, P, P, P, I, P]
+        L.vwb200_last_ipmatch_stats.argtypes = [C.POINTER(IpMatchStats)]
+        L.vwb200_remove_duplicate_matches.argtypes = [P, P, I, P, C.POINTER(I)]
         L.vwb200_corr_create.argtypes = [C.POINTER(CorrParams), C.POINTER(P)]
         L.vwb200_corr_set_inputs.argtypes = [P, P, I, I, Z, P, I, I, Z, P, Z, P, Z, I]
         L.vwb200_corr_rasterize.argtypes = [P, I, I, I, I, P, Z, I, P]
@@ -1071,3 +1077,164 @@ def epipolar_transformed_images(left_camera, right_camera, left_epi_camera, righ
             raise NoImplErr("epipolar_transformed_images: a ROI whose origin is not (0, 0) has no device form")
     return (camera_transform(left_image, left_camera, left_epi_camera, size=left_size, edge=EDGE_VALUE, edge_value=edge_value),
             camera_transform(right_image, right_camera, right_epi_camera, size=right_size, edge=EDGE_VALUE, edge_value=edge_value))
+
+
+# ---- exact interest point matching (InterestPoint/Matcher.h:415-509, Matcher.cc:33-195, MatcherIO.cc:248-365) --------------
+METRIC_L2, METRIC_HAMMING = 0, 1
+_METRICS = {"l2": METRIC_L2, "hamming": METRIC_HAMMING}
+
+
+class IpMatchStats(C.Structure):
+    _fields_ = [("pairs", C.c_longlong), ("matches", C.c_longlong), ("metric", C.c_int32), ("splits", C.c_int32)]
+
+
+def _points(desc, pol, what, on_device=None):
+    """(keep-alive, descriptor pointer, n, dim, pitch, polarity pointer, on_device) of an (n, dim) float32 descriptor list and
+    its n polarities"""
+    if len(desc.shape) != 2:
+        raise ArgumentErr(f"ip_match: {what} descriptors must be (n, dim), not {tuple(desc.shape)}")
+    if _is_torch(desc):
+        import torch
+        d = desc.to(torch.float32)
+        if d.stride(1) != 1 or d.shape[0] > 1 and d.stride(0) < d.shape[1]:
+            d = d.contiguous()
+        p = (pol if _is_torch(pol) else torch.as_tensor(np.asarray(pol))).to(device=d.device, dtype=torch.bool).to(torch.uint8).contiguous()
+        r = ((d, p), d.data_ptr(), d.shape[0], d.shape[1], max(d.stride(0), d.shape[1]), p.data_ptr(), 1)
+    else:
+        d = _np(desc, np.float32)
+        p = np.ascontiguousarray(np.asarray(pol).astype(bool), np.uint8)
+        r = ((d, p), d.ctypes.data, d.shape[0], d.shape[1], d.shape[1], p.ctypes.data, 0)
+    if tuple(p.shape) != (r[2],):
+        raise ArgumentErr(f"ip_match: {what} has {r[2]} descriptors but polarities of shape {tuple(p.shape)}")
+    if on_device is not None and r[6] != on_device:
+        raise ArgumentErr("ip_match: the inputs must all be numpy arrays or all be CUDA tensors")
+    return r
+
+
+def ip_match(desc1, pol1, desc2, pol2, threshold=0.5, metric="l2", distances=False):
+    """InterestPointMatcherSimple<L2NormMetric | HammingMetric, NullConstraint>(threshold) over two interest point lists given
+    as (n, dim) float32 descriptors and n polarities each (numpy arrays, or CUDA tensors on the current stream).  Returns the
+    int32 match index of every ip1 (-1: no match) where the inputs live; with distances=True also the reference's float64
+    first_pick / second_pick per ip1 (1e100 where none).  The matched pairs are (i, index[i]) for index[i] >= 0, in the
+    reference's order.  metric "hamming" compares the bytes static_cast<uint8>(value): a value outside (-1, 256) or NaN is
+    ArgumentErr, a dim above 2^21 NoImplErr.  Descriptors of unequal length are ArgumentErr."""
+    if metric not in _METRICS:
+        raise ArgumentErr(f"ip_match: unknown metric {metric!r} (l2 or hamming)")
+    k1, d1, n1, dim1, p1, q1, dev = _points(desc1, pol1, "ip1")
+    k2, d2, n2, dim2, p2, q2, _ = _points(desc2, pol2, "ip2", on_device=dev)
+    if dim1 != dim2 and n1 and n2:
+        raise ArgumentErr(f"ip_match: descriptors of unequal length ({dim1} and {dim2})")
+    dim = dim1 if n1 else dim2
+    index = _output(k1[0], (n1,), np.int32)
+    first = _output(k1[0], (n1,), np.float64) if distances else None
+    second = _output(k1[0], (n1,), np.float64) if distances else None
+    _check(lib().vwb200_ip_match(_METRICS[metric], d1, q1, n1, d2, q2, n2, dim, max(p1, dim), max(p2, dim), float(threshold), _ptr(index),
+                                 _ptr(first) if distances else None, _ptr(second) if distances else None, dev, _stream_ptr() if dev else None))
+    return (index, first, second) if distances else index
+
+
+def last_ipmatch_stats():
+    """what the last ip_match on this thread did: descriptor pairs scanned, the metric, the CTAs its candidate range was split
+    over (1: not split, 0: no candidates) and the matches kept"""
+    s = IpMatchStats()
+    lib().vwb200_last_ipmatch_stats(C.byref(s))
+    return {"pairs": int(s.pairs), "matches": int(s.matches), "metric": "hamming" if s.metric == METRIC_HAMMING else "l2",
+            "splits": int(s.splits)}
+
+
+def remove_duplicates(xy1, xy2):
+    """remove_duplicates(ip1, ip2) (Matcher.cc:151-195) on the (n, 2) float32 (x, y) of matched pairs: the int32 indices of the
+    pairs kept, in order.  Walking from the last pair to the first, a pair is dropped when its ip1 or its ip2 position was
+    already kept (-0.0 equals 0.0).  A NaN coordinate is ArgumentErr."""
+    a = _np(np.asarray(xy1.cpu() if _is_torch(xy1) else xy1), np.float32).reshape(-1, 2)
+    b = _np(np.asarray(xy2.cpu() if _is_torch(xy2) else xy2), np.float32).reshape(-1, 2)
+    if a.shape != b.shape:
+        raise ArgumentErr("remove_duplicates: Input vectors are not the same size.")
+    keep = np.empty(len(a), np.int32)
+    n = C.c_int()
+    _check(lib().vwb200_remove_duplicate_matches(a.ctypes.data, b.ctypes.data, len(a), keep.ctypes.data, C.byref(n)))
+    return keep[:n.value].copy()
+
+
+# the packed little-endian record of write_ip_record (MatcherIO.cc:248-263) ahead of its dim descriptor floats
+_IP_FIELDS = [("x", "<f4"), ("y", "<f4"), ("ix", "<i4"), ("iy", "<i4"), ("orientation", "<f4"), ("scale", "<f4"), ("interest", "<f4"),
+              ("polarity", "u1"), ("octave", "<u4"), ("scale_lvl", "<u4"), ("size", "<u8")]
+_IP_HEAD = np.dtype(_IP_FIELDS)          # 45 bytes, unaligned
+
+
+def _ip_dtype(dim):
+    return np.dtype(_IP_FIELDS + [("descriptor", "<f4", (dim,))])
+
+
+def interest_points(x, y, descriptor, polarity=None, scale=None, interest=None, orientation=None, octave=None, scale_lvl=None,
+                    ix=None, iy=None):
+    """an interest point list as the .vwip record array: InterestPoint(x, y, scale=1, interest=0, ori=0, pol=false, octave=0,
+    scale_lvl=0)'s defaults (ix, iy = int32(x), int32(y)) for the fields not given; descriptor is (n, dim)"""
+    d = np.asarray(descriptor, np.float32)
+    n = len(d)
+    rec = np.zeros(n, _ip_dtype(d.shape[1] if d.ndim == 2 else 0))
+    rec["x"], rec["y"] = x, y
+    rec["ix"] = np.asarray(x, np.float32).astype(np.int32) if ix is None else ix
+    rec["iy"] = np.asarray(y, np.float32).astype(np.int32) if iy is None else iy
+    rec["scale"] = 1.0 if scale is None else scale
+    for name, v in (("interest", interest), ("orientation", orientation), ("polarity", polarity), ("octave", octave), ("scale_lvl", scale_lvl)):
+        if v is not None:
+            rec[name] = v
+    rec["size"] = rec.dtype["descriptor"].shape[0]
+    rec["descriptor"] = d.reshape(n, -1)
+    return rec
+
+
+def _read_records(buf, offset, n):
+    if n == 0:
+        return np.zeros(0, _ip_dtype(0)), offset
+    if len(buf) < offset + _IP_HEAD.itemsize:
+        raise IOError("Failed to read interest point from file.")
+    dim = int(np.frombuffer(buf, "<u8", 1, offset + _IP_HEAD.itemsize - 8)[0])
+    dt = _ip_dtype(dim)
+    if len(buf) < offset + n * dt.itemsize:
+        raise IOError("Failed to read interest point from file.")
+    rec = np.frombuffer(buf, dt, n, offset).copy()
+    if np.any(rec["size"] != dim):
+        raise ValueError("interest point records with descriptors of different lengths are not supported")
+    return rec, offset + n * dt.itemsize
+
+
+def write_binary_ip_file(path, points):
+    """write_binary_ip_file (MatcherIO.cc:292-303): a u64 count, then the packed records of an interest_points() array"""
+    rec = np.asarray(points)
+    with open(path, "wb") as f:
+        f.write(np.uint64(len(rec)).astype("<u8").tobytes())
+        f.write(rec.tobytes())
+
+
+def read_binary_ip_file(path):
+    """read_binary_ip_file (MatcherIO.cc:305-322) as an interest_points() record array (every descriptor of one length)"""
+    with open(path, "rb") as f:
+        buf = f.read()
+    if len(buf) < 8:
+        return np.zeros(0, _ip_dtype(0))
+    return _read_records(buf, 8, int(np.frombuffer(buf, "<u8", 1, 0)[0]))[0]
+
+
+def write_binary_match_file(path, ip1, ip2):
+    """write_binary_match_file (MatcherIO.cc:344-366): the two u64 counts, the ip1 records, then the ip2 records"""
+    a, b = np.asarray(ip1), np.asarray(ip2)
+    if len(a) != len(b):
+        raise IOError("The vectors of matching interest points must have the same size.")
+    with open(path, "wb") as f:
+        f.write(np.array([len(a), len(b)], "<u8").tobytes())
+        f.write(a.tobytes())
+        f.write(b.tobytes())
+
+
+def read_binary_match_file(path):
+    """read_binary_match_file: (ip1, ip2) record arrays of a .match file"""
+    with open(path, "rb") as f:
+        buf = f.read()
+    if len(buf) < 16:
+        raise IOError(f"Failed to read {path} as a match file.")
+    n1, n2 = (int(v) for v in np.frombuffer(buf, "<u8", 2, 0))
+    ip1, off = _read_records(buf, 16, n1)
+    ip2, _ = _read_records(buf, off, n2)
+    return ip1, ip2

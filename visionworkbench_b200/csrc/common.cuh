@@ -258,6 +258,21 @@ int stereo_model_launch(const DispF* in, int w, int h, ptrdiff_t ip, const TriCa
 int universe_radius_launch(const double* in, int w, int h, ptrdiff_t ip, const double* origin, double near_r, double far_r, double* out,
                            ptrdiff_t op, unsigned long long* rejected, cudaStream_t st);
 
+// ---- K11: exact interest point matching (k11_ipmatch.cu); descriptor pitches in floats --------------------------------------
+// one query's summary over a set of candidates: the smallest distance, the lowest candidate index with it, and the
+// second-smallest distance (equal to best when best occurs twice); +inf / INT_MAX for none
+struct IpTop2 { float best; int j; float second; };
+struct IpMatchInfo {
+  int splits;                       // CTAs the candidate range was split over (0: no candidates)
+  unsigned long long matches;       // valid once the stream has synchronised
+  unsigned long long bad[2];        // Hamming: first invalid element index of desc1 / desc2 (row * dim + k), ~0 for none
+};
+// index / first / second: device outputs of n1 entries (first, second may be NULL).  Returns VWB200_EARG (with info->bad
+// set, stream synchronised) when a Hamming descriptor holds a value outside (-1, 256) or NaN.
+int ip_match_launch(int metric, const float* d1, ptrdiff_t p1, const uint8_t* pol1, int n1, const float* d2, ptrdiff_t p2,
+                    const uint8_t* pol2, int n2, int dim, double threshold, int* index, double* first, double* second, Arena& ar,
+                    cudaStream_t st, IpMatchInfo* info);
+
 // ---- host-side restatement-free logic -----------------------------------------------------------
 struct Box { int x0, y0, x1, y1; };
 struct HostZone { Box img; Box disp; };

@@ -16,6 +16,8 @@
 #include <cmath>
 #include <algorithm>
 #include <mutex>
+#include <set>
+#include <utility>
 #include <vector>
 
 namespace vwb200 {
@@ -1696,6 +1698,100 @@ int vwb200_fill_holes_grass(int pixel_type, const void* in, int w, int h, ptrdif
   if (pixel_type == VWB200_DISP_I32)
     return fill_holes_typed((const vwb200_dispi*)in, w, h, pitch, hole_fill_len, x0, y0, (vwb200_dispi*)out, ow, oh, opitch, on_device, stream);
   return fill_holes_typed((const DispF*)in, w, h, pitch, hole_fill_len, x0, y0, (DispF*)out, ow, oh, opitch, on_device, stream);
+}
+
+// ---- K11: InterestPointMatcherSimple (InterestPoint/Matcher.h:415-509) and remove_duplicates (Matcher.cc:151-195) -------------
+static thread_local vwb200_ipmatch_stats t_ipmatch_stats = {0, 0, 0, 0};
+
+int vwb200_last_ipmatch_stats(vwb200_ipmatch_stats* out) { if (!out) return VWB200_EARG; *out = t_ipmatch_stats; return VWB200_OK; }
+
+int vwb200_ip_match(int metric, const float* desc1, const uint8_t* pol1, int n1, const float* desc2, const uint8_t* pol2, int n2,
+                    int dim, ptrdiff_t pitch1, ptrdiff_t pitch2, double threshold, int32_t* match_index, double* first, double* second,
+                    int on_device, void* stream) {
+  t_ipmatch_stats = vwb200_ipmatch_stats{0, 0, metric, 0};
+  if (metric != VWB200_METRIC_L2 && metric != VWB200_METRIC_HAMMING) { set_error("ip_match: unknown metric %d", metric); return VWB200_EARG; }
+  if (n1 < 0 || n2 < 0 || dim < 0) { set_error("ip_match: bad sizes n1 %d, n2 %d, dim %d", n1, n2, dim); return VWB200_EARG; }
+  if (pitch1 < dim || pitch2 < dim) { set_error("ip_match: a pitch (%td, %td) is below the descriptor length %d", pitch1, pitch2, dim); return VWB200_EARG; }
+  if ((n1 > 0 && (!pol1 || !match_index || (dim > 0 && !desc1))) || (n2 > 0 && (!pol2 || (dim > 0 && !desc2)))) {
+    set_error("ip_match: null pointer");
+    return VWB200_EARG;
+  }
+  if (metric == VWB200_METRIC_HAMMING && 8ll * dim > (1ll << 24)) {
+    set_error("HammingMetric: descriptor length %d is above %d, where the float sum of bit counts stops being exact", dim, 1 << 21);
+    return VWB200_ENOIMPL;
+  }
+  // outputs: each other and every input (bytes, as rasters of one row per point)
+  struct Span { const void* p; int w, h; ptrdiff_t pitch; size_t px; };
+  const Span outs[3] = {{match_index, 1, n1, 1, 4}, {first, 1, n1, 1, 8}, {second, 1, n1, 1, 8}};
+  const Span ins[4] = {{desc1, dim, n1, pitch1, 4}, {desc2, dim, n2, pitch2, 4}, {pol1, 1, n1, 1, 1}, {pol2, 1, n2, 1, 1}};
+  for (int a = 0; a < 3; ++a) {
+    if (!outs[a].p) continue;
+    for (int b = a + 1; b < 3; ++b)
+      if (outs[b].p && rasters_overlap(outs[a].p, 1, n1, 1, outs[b].p, 1, n1, 1, outs[a].px, outs[b].px)) {
+        set_error("ip_match: the outputs overlap");
+        return VWB200_EARG;
+      }
+    for (const Span& s : ins)
+      if (s.p && rasters_overlap(outs[a].p, 1, n1, 1, s.p, s.w, s.h, s.pitch, outs[a].px, s.px)) {
+        set_error("ip_match: an output overlaps an input");
+        return VWB200_EARG;
+      }
+  }
+  VWB_TRY(ensure_device());
+  t_ipmatch_stats.pairs = (long long)n1 * n2;
+  if (n1 == 0) return VWB200_OK;
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
+  const float *d1 = nullptr, *d2 = nullptr;
+  const uint8_t *q1, *q2 = nullptr;
+  ptrdiff_t dp1 = dim, dp2 = dim, unused;
+  if (dim > 0) VWB_TRY(c.in(desc1, dim, n1, pitch1, on_device, &d1, &dp1));
+  VWB_TRY(c.in(pol1, 1, n1, 1, on_device, &q1, &unused));
+  if (n2 > 0) {
+    if (dim > 0) VWB_TRY(c.in(desc2, dim, n2, pitch2, on_device, &d2, &dp2));
+    VWB_TRY(c.in(pol2, 1, n2, 1, on_device, &q2, &unused));
+  }
+  int32_t* di; double *df = nullptr, *ds = nullptr;
+  VWB_TRY(c.out(match_index, 1, n1, 1, on_device, &di, &unused));
+  if (first) VWB_TRY(c.out(first, 1, n1, 1, on_device, &df, &unused));
+  if (second) VWB_TRY(c.out(second, 1, n1, 1, on_device, &ds, &unused));
+  IpMatchInfo info{0, 0, {~0ull, ~0ull}};
+  const int rc = ip_match_launch(metric, d1, dp1, q1, n1, d2, dp2, q2, n2, dim, threshold, di, df, ds, c.ar, c.st, &info);
+  if (rc == VWB200_EARG) {
+    const int list = info.bad[0] != ~0ull ? 0 : 1;
+    const unsigned long long e = info.bad[list];
+    const float* src = (list ? desc2 : desc1) + (ptrdiff_t)(e / dim) * (list ? pitch2 : pitch1) + (ptrdiff_t)(e % dim);
+    float v = 0.0f;
+    VWB_CUDA(cudaMemcpy(&v, src, sizeof v, on_device ? cudaMemcpyDeviceToHost : cudaMemcpyHostToHost));
+    set_error("HammingMetric: desc%d[%llu][%llu] = %g is not a byte value (outside (-1, 256) or NaN)", list + 1, e / dim, e % dim, (double)v);
+    return rc;
+  }
+  VWB_TRY(rc);
+  VWB_TRY(c.finish());
+  t_ipmatch_stats.splits = info.splits;
+  t_ipmatch_stats.matches = (long long)info.matches;
+  return VWB200_OK;
+}
+
+int vwb200_remove_duplicate_matches(const float* xy1, const float* xy2, int n, int32_t* keep, int* n_kept) {
+  if (n < 0 || !n_kept || (n > 0 && (!xy1 || !xy2 || !keep))) { set_error("remove_duplicates: bad arguments"); return VWB200_EARG; }
+  for (int i = 0; i < 2 * n; ++i)
+    if (std::isnan(xy1[i]) || std::isnan(xy2[i])) {
+      set_error("remove_duplicates: pair %d has a NaN coordinate, which has no place in an ordered set", i / 2);
+      return VWB200_EARG;
+    }
+  std::set<std::pair<float, float>> s1, s2;
+  int k = 0;
+  for (int j = n - 1; j >= 0; --j) {
+    const std::pair<float, float> a(xy1[2 * j], xy1[2 * j + 1]), b(xy2[2 * j], xy2[2 * j + 1]);
+    if (s1.count(a) || s2.count(b)) continue;
+    s1.insert(a);
+    s2.insert(b);
+    keep[k++] = j;
+  }
+  std::reverse(keep, keep + k);
+  *n_kept = k;
+  return VWB200_OK;
 }
 
 // ---- K10: triangulation (Stereo/StereoView.h, StereoModel.cc) through pinhole cameras ------------------------------------------
