@@ -281,7 +281,9 @@ int vwb200_stereo_model_points(const float* disparity, int w, int h, ptrdiff_t p
  * points, the largest error (exact) and the sum of the errors (summed in another order than the reference's raster order:
  * within 1e-12 relative); the mean error is error_sum / points.  tsai_iterations: the Newton-Raphson iterations of the last
  * vwb200_stereo_triangulate or vwb200_stereo_model_points (both rays of every triangulated pixel). */
-typedef struct { long long points, divergent; double max_error, error_sum; long long tsai_iterations; } vwb200_triangulation_stats;
+typedef struct { long long points, divergent; double max_error, error_sum; long long tsai_iterations;
+                 long long cahvor_iterations;   /* the CAHVOR Newton passes of the last vwb200_cahv_stereo_* call */
+} vwb200_triangulation_stats;
 int vwb200_last_triangulation_stats(vwb200_triangulation_stats* out);
 /* UniverseRadiusFunc(origin, near_radius, far_radius) applied to a w x h Vector3 image (StereoView.h:139-186): a point equal to
  * (0, 0, 0) (-0.0 included) becomes +0 and is not rejected; otherwise dist = norm_2(p - origin), and the point becomes +0
@@ -326,6 +328,46 @@ enum { VWB200_EDGE_VALUE = 2 };
 int vwb200_camera_transform(const vwb200_pinhole* src, const vwb200_pinhole* dst, int pixel_type, int interp, int edge, const float edge_value[2],
                             const void* in, int w, int h, ptrdiff_t pitch, int x0, int y0, void* out, int ow, int oh, ptrdiff_t opitch,
                             int on_device, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * JPL CAHV and CAHVOR cameras (Camera/CAHVModel.cc, CAHVORModel.cc, CameraTransform.h, StereoModel.cc:121-122).
+ * pixel_to_vector is normalize(cross(V - y*A, H - x*A)), negated when dot(cross(V, H), A) < 0; CAHVOR then removes the radial
+ * distortion with the reference's Newton loop (at most 20 passes, stopping when deriv <= 0 or after a step |du| < 1e-6).
+ * point_to_pixel is (dot(p, H), dot(p, V)) / dot(p, A) of p = point - C (CAHVOR: p + mu * lambda); it has no round-trip check,
+ * so these calls never return VWB200_EPROJECT.  Exactness: every double and float bit for bit the reference's (NaN payloads
+ * not kept).  VWB200_EARG, before the device is looked up, for a NULL pointer or an unknown model; the other arguments are
+ * checked as for the pinhole calls above.  CAHVORE is not supported.
+ * ------------------------------------------------------------------------------------------- */
+enum { VWB200_CAMERA_CAHV = 1, VWB200_CAMERA_CAHVOR = 2 };
+typedef struct {
+  int model;                                 /* VWB200_CAMERA_CAHV or VWB200_CAMERA_CAHVOR */
+  double C[3], A[3], H[3], V[3], O[3], R[3]; /* O and R are ignored for CAHV */
+} vwb200_cahv;
+/* epipolar(CAHVModel, CAHVModel) (CAHVModel.cc:297-337) on the host: both outputs share A, H, V and keep their source's C.
+ * The sources must be CAHV cameras (a CAHVOR camera is VWB200_EARG: linearize it first). */
+int vwb200_cahv_epipolar(const vwb200_cahv* cam0, const vwb200_cahv* cam1, vwb200_cahv* epi0, vwb200_cahv* epi1);
+/* linearize_camera(CAHVORModel, cahvor_image_size, cahv_image_size) (CAHVORModel.cc:460-547) on the host: the CAHV camera at
+ * the same C whose A is the normalised sum of 12 perimeter rays and whose H, V span the smallest field of view.  Sizes are
+ * (width, height).  cam must be a CAHVOR camera. */
+int vwb200_linearize_camera(const vwb200_cahv* cam, const int32_t cahvor_size[2], const int32_t cahv_size[2], vwb200_cahv* out);
+/* CAHVModel = PinholeModel (CAHVModel.cc:64-99) for a NULL-lens pinhole: VWB200_EARG for a Tsai lens (the conversion would drop
+ * it) and for a zero pixel pitch (the reference's ArgumentErr); the frame asserts and a singular matrix as for the pinhole
+ * calls. */
+int vwb200_pinhole_to_cahv(const vwb200_pinhole* pin, vwb200_cahv* out);
+/* camera_transform(image, src, dst, edge, interp) as vwb200_camera_transform, from a CAHV or CAHVOR src into a CAHV dst
+ * (a CAHVOR dst is VWB200_ENOIMPL); the same pixel types, interpolations, edges and window.  Cameras at different centers are
+ * VWB200_ELOGIC. */
+int vwb200_cahv_camera_transform(const vwb200_cahv* src, const vwb200_cahv* dst, int pixel_type, int interp, int edge, const float edge_value[2],
+                                 const void* in, int w, int h, ptrdiff_t pitch, int x0, int y0, void* out, int ow, int oh, ptrdiff_t opitch,
+                                 int on_device, void* stream);
+/* vwb200_stereo_triangulate and vwb200_stereo_model_points through CAHV or CAHVOR cameras (each may be either); the
+ * statistics are those of vwb200_last_triangulation_stats, with cahvor_iterations in place of tsai_iterations. */
+int vwb200_cahv_stereo_triangulate(int pixel_type, const void* disparity, int w, int h, ptrdiff_t pitch, int x0, int y0, int ow, int oh,
+                                   const vwb200_cahv* cam1, const vwb200_cahv* cam2, double angle_tol, double* xyz, ptrdiff_t xyz_pitch,
+                                   int on_device, void* stream);
+int vwb200_cahv_stereo_model_points(const float* disparity, int w, int h, ptrdiff_t pitch, const vwb200_cahv* cam1, const vwb200_cahv* cam2,
+                                    double angle_tol, double* xyz, ptrdiff_t xyz_pitch, double* error, ptrdiff_t error_pitch, int on_device,
+                                    void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Exact interest point matching: InterestPointMatcherSimple<L2NormMetric | HammingMetric, NullConstraint>::operator()

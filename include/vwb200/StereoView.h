@@ -7,13 +7,16 @@
 //                                                       (StereoModel.cc:254-309) on ImageView<PixelMask<Vector2f>>
 //   b200_universe_radius(points, origin, near, far)     UniverseRadiusFunc (StereoView.h:139-186) applied in place to an
 //                                                       ImageView<Vector3>; returns the rejected and total counts
-// The cameras must be camera::PinholeModel with a NULL or TSAI lens distortion; anything else throws NoImplErr.  Results are
-// bit for bit the reference's.
+// The cameras must both be camera::PinholeModel with a NULL or TSAI lens distortion, or each be a camera::CAHVModel or
+// camera::CAHVORModel; anything else, a pinhole with a CAHV-family camera included, throws NoImplErr.  Results are bit for bit
+// the reference's.
 #pragma once
 #ifdef VWB200_USE_REAL_VW
 #include <vw/Camera/CameraModel.h>
 #include <vw/Camera/LensDistortion.h>
 #include <vw/Camera/PinholeModel.h>
+#include <vw/Camera/CAHVModel.h>
+#include <vw/Camera/CAHVORModel.h>
 #endif
 #include <cfloat>
 #include <utility>
@@ -50,12 +53,47 @@ inline vwb200_pinhole pinhole_of(camera::CameraModel const* cam) {
   }
   return o;
 }
+
+// a CAHVModel or CAHVORModel as the ABI's camera; false for any other camera
+inline bool cahv_of(camera::CameraModel const* cam, vwb200_cahv* o) {
+  std::memset(o, 0, sizeof *o);
+  auto put = [](double* d, Vector3 const& v) { for (int i = 0; i < 3; ++i) d[i] = v[i]; };
+  if (camera::CAHVORModel const* c = dynamic_cast<camera::CAHVORModel const*>(cam)) {
+    o->model = VWB200_CAMERA_CAHVOR;
+    put(o->C, c->C); put(o->A, c->A); put(o->H, c->H); put(o->V, c->V); put(o->O, c->O); put(o->R, c->R);
+    return true;
+  }
+  if (camera::CAHVModel const* c = dynamic_cast<camera::CAHVModel const*>(cam)) {
+    o->model = VWB200_CAMERA_CAHV;
+    put(o->C, c->C); put(o->A, c->A); put(o->H, c->H); put(o->V, c->V);
+    return true;
+  }
+  return false;
+}
+
+// one camera of a triangulation: a pinhole, or a CAHV / CAHVOR camera
+struct TriCamera {
+  bool cahv;
+  vwb200_pinhole pin;
+  vwb200_cahv c;
+};
+inline TriCamera tri_camera(camera::CameraModel const* cam) {
+  TriCamera t;
+  std::memset(&t, 0, sizeof t);
+  t.cahv = cahv_of(cam, &t.c);
+  if (!t.cahv) t.pin = pinhole_of(cam);
+  return t;
+}
+// both cameras of one call are of one family
+inline void same_family(TriCamera const& a, TriCamera const& b) {
+  if (a.cahv != b.cahv) vw_throw(NoImplErr() << "b200 triangulation: a pinhole and a CAHV-family camera in one call have no device form");
+}
 }  // namespace b200_detail
 
 template <class ImageT>
 class B200StereoView : public ImageViewBase<B200StereoView<ImageT>> {
   ImageT m_disparity;
-  vwb200_pinhole m_cam1, m_cam2;
+  b200_detail::TriCamera m_cam1, m_cam2;
   double m_angle_tol;
 
 public:
@@ -64,7 +102,9 @@ public:
   typedef ProceduralPixelAccessor<B200StereoView<ImageT>> pixel_accessor;
 
   B200StereoView(ImageT const& disparity, camera::CameraModel const* cam1, camera::CameraModel const* cam2, double angle_tol = 0.0)
-    : m_disparity(disparity), m_cam1(b200_detail::pinhole_of(cam1)), m_cam2(b200_detail::pinhole_of(cam2)), m_angle_tol(angle_tol) {}
+    : m_disparity(disparity), m_cam1(b200_detail::tri_camera(cam1)), m_cam2(b200_detail::tri_camera(cam2)), m_angle_tol(angle_tol) {
+    b200_detail::same_family(m_cam1, m_cam2);
+  }
 
   int32 cols() const { return m_disparity.cols(); }
   int32 rows() const { return m_disparity.rows(); }
@@ -81,9 +121,15 @@ public:
     typedef typename ImageT::pixel_type dpixel;
     static_assert(sizeof(dpixel) == 12, "disparity pixels must be {dx, dy, valid} triples of 4-byte values");
     ImageView<Vector3> win(bbox.width(), bbox.height());
-    b200_detail::check(vwb200_stereo_triangulate(b200_detail::DispPixel<dpixel>::type, m_disparity.data(), m_disparity.cols(), m_disparity.rows(),
-                                                 m_disparity.rstride(), bbox.min()[0], bbox.min()[1], win.cols(), win.rows(), &m_cam1, &m_cam2,
-                                                 m_angle_tol, reinterpret_cast<double*>(win.data()), win.rstride(), /*on_device=*/0, nullptr));
+    if (m_cam1.cahv)
+      b200_detail::check(vwb200_cahv_stereo_triangulate(b200_detail::DispPixel<dpixel>::type, m_disparity.data(), m_disparity.cols(),
+                                                        m_disparity.rows(), m_disparity.rstride(), bbox.min()[0], bbox.min()[1], win.cols(),
+                                                        win.rows(), &m_cam1.c, &m_cam2.c, m_angle_tol, reinterpret_cast<double*>(win.data()),
+                                                        win.rstride(), /*on_device=*/0, nullptr));
+    else
+      b200_detail::check(vwb200_stereo_triangulate(b200_detail::DispPixel<dpixel>::type, m_disparity.data(), m_disparity.cols(), m_disparity.rows(),
+                                                   m_disparity.rstride(), bbox.min()[0], bbox.min()[1], win.cols(), win.rows(), &m_cam1.pin, &m_cam2.pin,
+                                                   m_angle_tol, reinterpret_cast<double*>(win.data()), win.rstride(), /*on_device=*/0, nullptr));
     return prerasterize_type(win, -bbox.min()[0], -bbox.min()[1], cols(), rows());
   }
 
@@ -98,20 +144,27 @@ inline B200StereoView<ImageT> b200_stereo_triangulate(ImageT const& disparity, c
 }
 
 class B200StereoModel {
-  vwb200_pinhole m_cam1, m_cam2;
+  b200_detail::TriCamera m_cam1, m_cam2;
   double m_angle_tol;
 
 public:
   B200StereoModel(camera::CameraModel const* camera_model1, camera::CameraModel const* camera_model2, double angle_tol = 0.0)
-    : m_cam1(b200_detail::pinhole_of(camera_model1)), m_cam2(b200_detail::pinhole_of(camera_model2)), m_angle_tol(angle_tol) {}
+    : m_cam1(b200_detail::tri_camera(camera_model1)), m_cam2(b200_detail::tri_camera(camera_model2)), m_angle_tol(angle_tol) {
+    b200_detail::same_family(m_cam1, m_cam2);
+  }
 
   // StereoModel::operator()(disparity_map, error); the statistics the reference prints are vwb200_last_triangulation_stats
   ImageView<Vector3> operator()(ImageView<PixelMask<Vector2f>> const& disparity_map, ImageView<double>& error) const {
     ImageView<Vector3> xyz(disparity_map.cols(), disparity_map.rows());
     error.set_size(disparity_map.cols(), disparity_map.rows());
-    b200_detail::check(vwb200_stereo_model_points(reinterpret_cast<const float*>(disparity_map.data()), disparity_map.cols(),
-                                                  disparity_map.rows(), disparity_map.rstride(), &m_cam1, &m_cam2, m_angle_tol,
-                                                  reinterpret_cast<double*>(xyz.data()), xyz.rstride(), error.data(), error.rstride(), 0, nullptr));
+    const float* d = reinterpret_cast<const float*>(disparity_map.data());
+    double* p = reinterpret_cast<double*>(xyz.data());
+    if (m_cam1.cahv)
+      b200_detail::check(vwb200_cahv_stereo_model_points(d, disparity_map.cols(), disparity_map.rows(), disparity_map.rstride(), &m_cam1.c, &m_cam2.c,
+                                                         m_angle_tol, p, xyz.rstride(), error.data(), error.rstride(), 0, nullptr));
+    else
+      b200_detail::check(vwb200_stereo_model_points(d, disparity_map.cols(), disparity_map.rows(), disparity_map.rstride(), &m_cam1.pin, &m_cam2.pin,
+                                                    m_angle_tol, p, xyz.rstride(), error.data(), error.rstride(), 0, nullptr));
     return xyz;
   }
 };

@@ -15,8 +15,9 @@
 //   Zero/ConstantEdgeExtension, Bilinear/Bicubic/NearestPixelInterpolation   tag types only (EdgeExtension.tcc, Interpolation.h)
 //   ValueEdgeExtension<PixelT>  Image/EdgeExtension.h:66-76 (the edge pixel only)
 //   Vector3                     Math/Vector.h           (3 doubles)
-//   camera::CameraModel, PinholeModel, NullLensDistortion, TsaiLensDistortion
-//                               Camera/CameraModel.h, PinholeModel.h:158-261, LensDistortion.h (constructors and accessors only)
+//   camera::CameraModel, PinholeModel, NullLensDistortion, TsaiLensDistortion, CAHVModel, CAHVORModel
+//                               Camera/CameraModel.h, PinholeModel.h:158-261, LensDistortion.h (constructors and accessors only),
+//                               CAHVModel.h and CAHVORModel.h (the public vectors and constructors)
 //   camera::PointToPixelErr     Camera/CameraModel.h:229
 //   ip::InterestPoint           InterestPoint/InterestPoint.h:45-110 (fields and constructor; descriptor as std::vector<float>)
 //   ip::L2NormMetric, HammingMetric, NullConstraint   InterestPoint/Matcher.h (tag types only)
@@ -283,6 +284,23 @@ public:
   void coordinate_frame(Vector3& u, Vector3& v, Vector3& w) const { u = m_u; v = m_v; w = m_w; }
   double pixel_pitch() const { return m_pixel_pitch; }
   LensDistortion const* lens_distortion() const { return m_distortion.get(); }
+};
+class CAHVModel : public CameraModel {                                                         // Camera/CAHVModel.h: public C, A, H, V
+public:
+  Vector3 C, A, H, V;
+  CAHVModel() {}
+  CAHVModel(Vector3 const& C_vec, Vector3 const& A_vec, Vector3 const& H_vec, Vector3 const& V_vec) : C(C_vec), A(A_vec), H(H_vec), V(V_vec) {}
+  std::string type() const override { return "CAHV"; }
+  Vector3 camera_center(Vector2<double> const& = Vector2<double>()) const { return C; }
+};
+class CAHVORModel : public CameraModel {                                                       // Camera/CAHVORModel.h: C, A, H, V, O, R
+public:
+  Vector3 C, A, H, V, O, R;
+  CAHVORModel() {}
+  CAHVORModel(Vector3 const& C_vec, Vector3 const& A_vec, Vector3 const& H_vec, Vector3 const& V_vec, Vector3 const& O_vec, Vector3 const& R_vec)
+    : C(C_vec), A(A_vec), H(H_vec), V(V_vec), O(O_vec), R(R_vec) {}
+  std::string type() const override { return "CAHVOR"; }
+  Vector3 camera_center(Vector2<double> const& = Vector2<double>()) const { return C; }
 };
 }  // namespace camera
 

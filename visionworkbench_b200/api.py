@@ -33,6 +33,7 @@ library) or torch CUDA tensors (used in place, results returned as torch CUDA te
 """
 import ctypes as C
 import os
+import re
 
 import numpy as np
 
@@ -80,6 +81,10 @@ class NoDeviceErr(VwError):
 
 class PointToPixelErr(VwError):
     """vw::camera::PointToPixelErr: point_to_pixel's round-trip check failed (VWB200_EPROJECT)"""
+
+
+class IOErr(VwError):
+    """vw::IOErr: a camera file could not be read"""
 
 
 _ERR = {-1: ArgumentErr, -2: MathErr, -3: LogicErr, -4: NoImplErr, -5: CudaErr, -6: NoDeviceErr, -7: MemoryError, -8: PointToPixelErr}
@@ -156,6 +161,13 @@ def lib():
         L.vwb200_pinhole_epipolar.argtypes = [PH, PH, PH, PH]
         L.vwb200_resize_epipolar_cameras_to_fit.argtypes = [PH, PH, PH, PH, P, P, P, P, P]
         L.vwb200_camera_transform.argtypes = [PH, PH, I, I, I, P, P, I, I, Z, I, I, P, I, I, Z, I, P]
+        CH = C.POINTER(Cahv)
+        L.vwb200_cahv_epipolar.argtypes = [CH, CH, CH, CH]
+        L.vwb200_linearize_camera.argtypes = [CH, P, P, CH]
+        L.vwb200_pinhole_to_cahv.argtypes = [PH, CH]
+        L.vwb200_cahv_camera_transform.argtypes = [CH, CH, I, I, I, P, P, I, I, Z, I, I, P, I, I, Z, I, P]
+        L.vwb200_cahv_stereo_triangulate.argtypes = [I, P, I, I, Z, I, I, I, I, CH, CH, D, P, Z, I, P]
+        L.vwb200_cahv_stereo_model_points.argtypes = [P, I, I, Z, CH, CH, D, P, Z, P, Z, I, P]
         L.vwb200_ip_match.argtypes = [I, P, P, I, P, P, I, I, Z, Z, D, P, P, P, I, P]
         L.vwb200_last_ipmatch_stats.argtypes = [C.POINTER(IpMatchStats)]
         L.vwb200_remove_duplicate_matches.argtypes = [P, P, I, P, C.POINTER(I)]
@@ -743,11 +755,17 @@ class PinholeModel:
 def stereo_triangulate(disparity, cam1, cam2, bbox=None, angle_tol=0.0):
     """stereo_triangulate(disparity, cam1, cam2) (Stereo/StereoView.h:74-130) rasterised over bbox (x0, y0, x1, y1) or a BBox2i
     inside the image (None: the whole image).  Pixel (i, j) triangulates (i, j) against (i, j) + (double)disparity through
-    StereoModel(cam1, cam2, angle_tol); invalid pixels give (0, 0, 0).  int32 or float32 (rows, cols, 3), numpy or CUDA;
+    StereoModel(cam1, cam2, angle_tol); invalid pixels give (0, 0, 0).  The cameras are both PinholeModels, or each a CAHVModel or
+    a CAHVORModel (a pinhole with a CAHV-family camera is NoImplErr).  int32 or float32 (rows, cols, 3), numpy or CUDA;
     returns a (y1 - y0, x1 - x0, 3) float64 raster of the same kind."""
     t, ptr, cols, rows, pitch, dev, dt = _disparity_in(disparity)
     x0, y0, x1, y1 = _bbox(bbox) if bbox is not None else (0, 0, cols, rows)
     out = _output(t, (max(y1 - y0, 0), max(x1 - x0, 0), 3), np.float64)
+    if _family("stereo_triangulate", cam1, cam2) == "cahv":
+        _check(lib().vwb200_cahv_stereo_triangulate(_ptype(dt), ptr, cols, rows, pitch, x0, y0, x1 - x0, y1 - y0, C.byref(cam1._struct()),
+                                                    C.byref(cam2._struct()), float(angle_tol), _ptr(out), x1 - x0, dev,
+                                                    _stream_ptr() if dev else None))
+        return out
     c1, c2 = cam1._struct(), cam2._struct()
     _check(lib().vwb200_stereo_triangulate(_ptype(dt), ptr, cols, rows, pitch, x0, y0, x1 - x0, y1 - y0, C.byref(c1), C.byref(c2),
                                            float(angle_tol), _ptr(out), x1 - x0, dev, _stream_ptr() if dev else None))
@@ -762,20 +780,22 @@ def stereo_model_points(disparity, cam1, cam2, angle_tol=0.0):
     if dt != np.float32:
         raise ArgumentErr("StereoModel takes a float32 (PixelMask<Vector2f>) disparity")
     xyz, err = _output(t, (rows, cols, 3), np.float64), _output(t, (rows, cols), np.float64)
+    fn = lib().vwb200_cahv_stereo_model_points if _family("StereoModel", cam1, cam2) == "cahv" else lib().vwb200_stereo_model_points
     c1, c2 = cam1._struct(), cam2._struct()
-    _check(lib().vwb200_stereo_model_points(ptr, cols, rows, pitch, C.byref(c1), C.byref(c2), float(angle_tol), _ptr(xyz), cols, _ptr(err),
-                                            cols, dev, _stream_ptr() if dev else None))
+    _check(fn(ptr, cols, rows, pitch, C.byref(c1), C.byref(c2), float(angle_tol), _ptr(xyz), cols, _ptr(err), cols, dev,
+              _stream_ptr() if dev else None))
     return xyz, err
 
 
 class TriangulationStats(C.Structure):
     _fields_ = [("points", C.c_longlong), ("divergent", C.c_longlong), ("max_error", C.c_double), ("error_sum", C.c_double),
-                ("tsai_iterations", C.c_longlong)]
+                ("tsai_iterations", C.c_longlong), ("cahvor_iterations", C.c_longlong)]
 
 
 def last_triangulation_stats():
     """what the last stereo_model_points on this thread reports: points, divergent, max_error, error_sum (mean error =
-    error_sum / points), and the Tsai Newton-Raphson iterations of the last stereo_triangulate or stereo_model_points"""
+    error_sum / points), and the Tsai Newton-Raphson (pinhole cameras) or CAHVOR Newton (CAHV cameras) iterations of the last
+    stereo_triangulate or stereo_model_points"""
     s = TriangulationStats()
     lib().vwb200_last_triangulation_stats(C.byref(s))
     return {k: getattr(s, k) for k, _ in TriangulationStats._fields_}
@@ -1019,7 +1039,12 @@ PIXEL_GRAY_F32, PIXEL_MASK_F32 = 0, 1
 def epipolar(cam0, cam1):
     """epipolar(cam0, cam1, epi0, epi1) (Camera/PinholeModel.cc:679-732): two rectified PinholeModels at the sources' centers,
     sharing one rotation (baseline as u), the mean focal length, point offset and pixel pitch, the NULL lens and the default
-    u, v, w frame.  Host arithmetic, bit for bit the reference's; coincident centers give NaN cameras."""
+    u, v, w frame.  Host arithmetic, bit for bit the reference's; coincident centers give NaN cameras.  For two CAHVModels,
+    epipolar(CAHVModel, CAHVModel) (Camera/CAHVModel.cc:297-337): two CAHVModels at the sources' centers sharing A, H and V."""
+    if _family("epipolar", cam0, cam1) == "cahv":
+        a, b = Cahv(), Cahv()
+        _check(lib().vwb200_cahv_epipolar(C.byref(cam0._struct()), C.byref(cam1._struct()), C.byref(a), C.byref(b)))
+        return _cahv_from_struct(a), _cahv_from_struct(b)
     a, b = Pinhole(), Pinhole()
     _check(lib().vwb200_pinhole_epipolar(C.byref(cam0._struct()), C.byref(cam1._struct()), C.byref(a), C.byref(b)))
     return PinholeModel._from_struct(a), PinholeModel._from_struct(b)
@@ -1049,7 +1074,9 @@ def camera_transform(image, src_camera, dst_camera, bbox=None, size=None, edge=E
     interpolation, zero or constant edges -- or PixelMask<float> (rows, cols, 2) {value, valid} -- bilinear, with zero,
     constant or value edges (edge_value {value, valid}, default PixelMask<float>() = (0, 0)); numpy or CUDA.  Bit for bit the
     reference's where both reversed coordinates are finite with |c| < 2^30; 0 ({0, 0}) elsewhere.  PointToPixelErr, naming the
-    first failing pixel, where the reference throws.  Returns a new raster where the image lives."""
+    first failing pixel, where the reference throws.  Returns a new raster where the image lives.  The cameras are both
+    PinholeModels, or a CAHVModel / CAHVORModel src and a CAHVModel dst (no check, so no PointToPixelErr); a pinhole with a
+    CAHV-family camera is NoImplErr."""
     masked = len(image.shape) == 3
     if masked and image.shape[2] != 2 or len(image.shape) not in (2, 3):
         raise ArgumentErr("camera_transform: the image must be float32 (rows, cols) or PixelMask<float> (rows, cols, 2)")
@@ -1060,9 +1087,9 @@ def camera_transform(image, src_camera, dst_camera, bbox=None, size=None, edge=E
         x0, y0, x1, y1 = _bbox(bbox) if bbox is not None else (0, 0, cols, rows)
     ev = (C.c_float * 2)(*(edge_value if edge_value is not None else (0.0, 0.0)))
     out = _output(t, (max(y1 - y0, 0), max(x1 - x0, 0)) + ((2,) if masked else ()), np.float32)
-    _check(lib().vwb200_camera_transform(C.byref(src_camera._struct()), C.byref(dst_camera._struct()), PIXEL_MASK_F32 if masked else PIXEL_GRAY_F32,
-                                         int(interp), int(edge), ev, ptr, cols, rows, pitch, x0, y0, _ptr(out), x1 - x0, y1 - y0, x1 - x0, dev,
-                                         _stream_ptr() if dev else None))
+    fn = lib().vwb200_cahv_camera_transform if _family("camera_transform", src_camera, dst_camera) == "cahv" else lib().vwb200_camera_transform
+    _check(fn(C.byref(src_camera._struct()), C.byref(dst_camera._struct()), PIXEL_MASK_F32 if masked else PIXEL_GRAY_F32, int(interp), int(edge),
+              ev, ptr, cols, rows, pitch, x0, y0, _ptr(out), x1 - x0, y1 - y0, x1 - x0, dev, _stream_ptr() if dev else None))
     return out
 
 
@@ -1077,6 +1104,203 @@ def epipolar_transformed_images(left_camera, right_camera, left_epi_camera, righ
             raise NoImplErr("epipolar_transformed_images: a ROI whose origin is not (0, 0) has no device form")
     return (camera_transform(left_image, left_camera, left_epi_camera, size=left_size, edge=EDGE_VALUE, edge_value=edge_value),
             camera_transform(right_image, right_camera, right_epi_camera, size=right_size, edge=EDGE_VALUE, edge_value=edge_value))
+
+
+# ---- CAHV / CAHVOR cameras (Camera/CAHVModel.cc, CAHVORModel.cc, CameraTransform.h:185-225, EpipolarUtils.cc:148-222) ---------
+CAMERA_CAHV, CAMERA_CAHVOR = 1, 2
+
+
+class Cahv(C.Structure):
+    _fields_ = [("model", C.c_int), ("C", C.c_double * 3), ("A", C.c_double * 3), ("H", C.c_double * 3), ("V", C.c_double * 3),
+                ("O", C.c_double * 3), ("R", C.c_double * 3)]
+
+
+def _vec3(v):
+    return tuple(float(x) for x in v)
+
+
+_WS = " \t\n\v\f\r"
+_DOUBLE = re.compile(r"[+-]?(\d*)(?:\.(\d*))?")
+_EXPONENT = re.compile(r"[eE][+-]?(\d*)")
+
+
+class _TextIn:
+    """the std::istream reads of the reference's camera readers (C locale): ignore(n, delim), >> char and >> double.  A double
+    is what num_get accumulates -- sign, digits, a decimal point, an exponent -- converted as a whole, so "nan", "inf", hex,
+    a bare "." or "1e" and a value that overflows fail; any failure is IOErr, as the reference's failbit exception is."""
+
+    def __init__(self, text, what):
+        self.t, self.p, self.what = text, 0, what
+
+    def fail(self, msg="Could not read file"):
+        raise IOErr(f"{self.what}: {msg}")
+
+    def ignore(self, n, delim):
+        k = self.t.find(delim, self.p, self.p + n)
+        self.p = min(len(self.t), self.p + n) if k < 0 else k + 1
+
+    def _skip(self):
+        while self.p < len(self.t) and self.t[self.p] in _WS:
+            self.p += 1
+        if self.p >= len(self.t):
+            self.fail()
+
+    def char(self):
+        self._skip()
+        self.p += 1
+        return self.t[self.p - 1]
+
+    def double(self):
+        self._skip()
+        m = _DOUBLE.match(self.t, self.p)
+        end, digits = m.end(), (m.group(1) or "") + (m.group(2) or "")
+        if digits:
+            e = _EXPONENT.match(self.t, end)
+            if e:
+                end = e.end()
+                if not e.group(1):
+                    self.fail()
+        if not digits:
+            self.fail()
+        v = float(self.t[self.p:end])
+        if v in (float("inf"), float("-inf")):
+            self.fail()
+        self.p = end
+        return v
+
+
+def _read_vectors(path, names, what):
+    """the readers of CAHVModel.cc:194-231 and CAHVORModel.cc:30-80: skip to "C" followed by "=", then the vectors, each after
+    its letter and "="""
+    with open(path) as f:
+        s = _TextIn(f.read(), what)
+    while True:
+        s.ignore(1024, "C")
+        if s.char() == "=":
+            break
+    out = [tuple(s.double() for _ in range(3))]
+    for name in names[1:]:
+        if s.char() != name or s.char() != "=":
+            s.fail(f"Could not read {name} vector")
+        out.append(tuple(s.double() for _ in range(3)))
+    return out
+
+
+def _write_vectors(path, pairs):
+    with open(path, "w") as f:
+        for name, v in pairs:
+            f.write(f"{name} = " + " ".join(format(x, ".20g") for x in v) + "\n")
+
+
+class CAHVModel:
+    """camera::CAHVModel(C, A, H, V) (Camera/CAHVModel.h): the four vectors as public fields.  read() / write() use the
+    reference's text format (any leading text is skipped up to "C ="; written with 20 significant digits)."""
+    type_name = "CAHV"
+
+    def __init__(self, C=(0, 0, 0), A=(0, 0, 0), H=(0, 0, 0), V=(0, 0, 0)):
+        self.C, self.A, self.H, self.V = _vec3(C), _vec3(A), _vec3(H), _vec3(V)
+
+    def camera_center(self, pix=None):
+        return self.C
+
+    def type(self):
+        return self.type_name
+
+    @classmethod
+    def read(cls, path):
+        return cls(*_read_vectors(path, "CAHV", "CAHVModel"))
+
+    def write(self, path):
+        _write_vectors(path, zip("CAHV", (self.C, self.A, self.H, self.V)))
+
+    @classmethod
+    def from_pinhole(cls, pinhole):
+        """CAHVModel = PinholeModel (CAHVModel.cc:64-99) of a NULL-lens pinhole, on the host"""
+        out = Cahv()
+        _check(lib().vwb200_pinhole_to_cahv(C.byref(pinhole._struct()), C.byref(out)))
+        return _cahv_from_struct(out)
+
+    def _struct(self):
+        s = Cahv()
+        s.model = CAMERA_CAHV
+        s.C[:], s.A[:], s.H[:], s.V[:] = self.C, self.A, self.H, self.V
+        return s
+
+    def __repr__(self):
+        return f"{type(self).__name__}(C={self.C}, A={self.A}, H={self.H}, V={self.V})"
+
+
+class CAHVORModel(CAHVModel):
+    """camera::CAHVORModel(C, A, H, V, O, R) (Camera/CAHVORModel.h): CAHV plus the optical axis O and the radial distortion
+    terms R"""
+    type_name = "CAHVOR"
+
+    def __init__(self, C=(0, 0, 0), A=(0, 0, 0), H=(0, 0, 0), V=(0, 0, 0), O=(0, 0, 0), R=(0, 0, 0)):
+        super().__init__(C, A, H, V)
+        self.O, self.R = _vec3(O), _vec3(R)
+
+    @classmethod
+    def read(cls, path):
+        return cls(*_read_vectors(path, "CAHVOR", "CAHVORModel"))
+
+    def write(self, path):
+        _write_vectors(path, zip("CAHVOR", (self.C, self.A, self.H, self.V, self.O, self.R)))
+
+    def _struct(self):
+        s = super()._struct()
+        s.model = CAMERA_CAHVOR
+        s.O[:], s.R[:] = self.O, self.R
+        return s
+
+    def __repr__(self):
+        return f"CAHVORModel(C={self.C}, A={self.A}, H={self.H}, V={self.V}, O={self.O}, R={self.R})"
+
+
+def _cahv_from_struct(s):
+    if s.model == CAMERA_CAHVOR:
+        return CAHVORModel(s.C[:], s.A[:], s.H[:], s.V[:], s.O[:], s.R[:])
+    return CAHVModel(s.C[:], s.A[:], s.H[:], s.V[:])
+
+
+def _family(what, *cams):
+    """"pinhole" when every camera is a PinholeModel, "cahv" when every one is a CAHVModel / CAHVORModel; NoImplErr for a mix"""
+    if all(isinstance(c, PinholeModel) for c in cams):
+        return "pinhole"
+    if all(isinstance(c, CAHVModel) for c in cams):
+        return "cahv"
+    raise NoImplErr(f"{what}: pinhole and CAHV-family cameras in one call have no device form")
+
+
+def linearize_camera(camera_model, cahvor_image_size, cahv_image_size):
+    """linearize_camera(CAHVORModel, cahvor_image_size, cahv_image_size) (Camera/CAHVORModel.cc:460-547), on the host: the
+    CAHVModel at the same center with A the normalised sum of 12 perimeter rays and H, V spanning the smaller field of view.
+    Sizes are (width, height)."""
+    if not isinstance(camera_model, CAHVORModel):
+        raise ArgumentErr("linearize_camera takes a CAHVORModel")
+    out = Cahv()
+    _check(lib().vwb200_linearize_camera(C.byref(camera_model._struct()), (C.c_int32 * 2)(*cahvor_image_size), (C.c_int32 * 2)(*cahv_image_size),
+                                         C.byref(out)))
+    return _cahv_from_struct(out)
+
+
+def linearize_camera_transform(image, camera_model, edge=EDGE_ZERO, interp=INTERP_BILINEAR, edge_value=None):
+    """linearize_camera_transform(image, cahvor[, edge, interp]) (Camera/CameraTransform.h:185-225): the image resampled from
+    camera_model into linearize_camera(camera_model, size, size) of its own size (cols, rows)"""
+    rows, cols = image.shape[0], image.shape[1]
+    lin = linearize_camera(camera_model, (cols, rows), (cols, rows))
+    return camera_transform(image, camera_model, lin, edge=edge, interp=interp, edge_value=edge_value)
+
+
+def epipolar_transformed_cahv_images(left_camera, right_camera, left_epi_camera, right_epi_camera, left_image, right_image,
+                                     edge_value=(0.0, 0.0)):
+    """the CAHV and CAHVOR branches of epipolar_transformed_cahv_images (Camera/EpipolarUtils.cc:148-222): both PixelMask<float>
+    (rows, cols, 2) images resampled from their CAHV / CAHVOR cameras into the epipolar CAHV cameras at their own size,
+    bilinear, ValueEdgeExtension(edge_value)"""
+    for c in (left_epi_camera, right_epi_camera):
+        if type(c) is not CAHVModel:
+            raise ArgumentErr("epipolar_transformed_cahv_images: the epipolar cameras must be CAHVModels")
+    return (camera_transform(left_image, left_camera, left_epi_camera, edge=EDGE_VALUE, edge_value=edge_value),
+            camera_transform(right_image, right_camera, right_epi_camera, edge=EDGE_VALUE, edge_value=edge_value))
 
 
 # ---- exact interest point matching (InterestPoint/Matcher.h:415-509, Matcher.cc:33-195, MatcherIO.cc:248-365) --------------

@@ -1906,14 +1906,40 @@ static int cameras_open(const char* what, const vwb200_pinhole* cam1, const vwb2
   return ensure_device();
 }
 
-// zeroed device statistics of one call, copied to host[5] at finish()
-static int tri_stats_open(AbiCall& c, unsigned long long** d) {
-  VWB_TRY(c.ar.alloc(d, 5));
-  VWB_CUDA(cudaMemsetAsync(*d, 0, 5 * sizeof(unsigned long long), c.st));
+// n (5, or 6 with the CAHVOR counter) zeroed device statistics of one call
+static int tri_stats_open(AbiCall& c, unsigned long long** d, int n = 5) {
+  VWB_TRY(c.ar.alloc(d, n));
+  VWB_CUDA(cudaMemsetAsync(*d, 0, n * sizeof(unsigned long long), c.st));
   return VWB200_OK;
 }
 
 int vwb200_last_triangulation_stats(vwb200_triangulation_stats* out) { if (!out) return VWB200_EARG; *out = t_tri_stats; return VWB200_OK; }
+
+// the raster checks of stereo_triangulate (after the cameras')
+static int triangulate_args(const char* what, const void* disparity, int w, int h, ptrdiff_t pitch, int x0, int y0, int ow, int oh,
+                            const double* xyz, ptrdiff_t xyz_pitch) {
+  if (w <= 0 || h <= 0 || pitch < w) { set_error("%s: bad input size %d x %d, pitch %td", what, w, h, pitch); return VWB200_EARG; }
+  if (ow <= 0 || oh <= 0 || xyz_pitch < ow) { set_error("%s: bad output size %d x %d, pitch %td", what, ow, oh, xyz_pitch); return VWB200_EARG; }
+  if (x0 < 0 || y0 < 0 || x0 > w - ow || y0 > h - oh) {
+    set_error("%s: the window (%d, %d, %d, %d) leaves the %d x %d input", what, x0, y0, ow, oh, w, h);
+    return VWB200_EARG;
+  }
+  if (rasters_overlap(disparity, w, h, pitch, xyz, ow, oh, xyz_pitch, 12, 24)) { set_error("%s: xyz overlaps the disparity", what); return VWB200_EARG; }
+  return VWB200_OK;
+}
+
+// the raster checks of StereoModel's image form (after the cameras')
+static int model_points_args(const char* what, const float* disparity, int w, int h, ptrdiff_t pitch, const double* xyz, ptrdiff_t xyz_pitch,
+                             const double* error, ptrdiff_t error_pitch) {
+  if (w <= 0 || h <= 0 || pitch < w) { set_error("%s: bad input size %d x %d, pitch %td", what, w, h, pitch); return VWB200_EARG; }
+  if (xyz_pitch < w || error_pitch < w) { set_error("%s: output pitches %td, %td are below the width %d", what, xyz_pitch, error_pitch, w); return VWB200_EARG; }
+  if (rasters_overlap(disparity, w, h, pitch, xyz, w, h, xyz_pitch, 12, 24) || rasters_overlap(disparity, w, h, pitch, error, w, h, error_pitch, 12, 8) ||
+      rasters_overlap(xyz, w, h, xyz_pitch, error, w, h, error_pitch, 24, 8)) {
+    set_error("%s: the disparity, xyz and error rasters overlap", what);
+    return VWB200_EARG;
+  }
+  return VWB200_OK;
+}
 
 int vwb200_stereo_triangulate(int pixel_type, const void* disparity, int w, int h, ptrdiff_t pitch, int x0, int y0, int ow, int oh,
                               const vwb200_pinhole* cam1, const vwb200_pinhole* cam2, double angle_tol, double* xyz, ptrdiff_t xyz_pitch,
@@ -1924,13 +1950,7 @@ int vwb200_stereo_triangulate(int pixel_type, const void* disparity, int w, int 
   if (pixel_type != VWB200_DISP_I32 && pixel_type != VWB200_DISP_F32) { set_error("%s: unknown pixel type %d", what, pixel_type); return VWB200_EARG; }
   VWB_TRY(pinhole_check(what, cam1));
   VWB_TRY(pinhole_check(what, cam2));
-  if (w <= 0 || h <= 0 || pitch < w) { set_error("%s: bad input size %d x %d, pitch %td", what, w, h, pitch); return VWB200_EARG; }
-  if (ow <= 0 || oh <= 0 || xyz_pitch < ow) { set_error("%s: bad output size %d x %d, pitch %td", what, ow, oh, xyz_pitch); return VWB200_EARG; }
-  if (x0 < 0 || y0 < 0 || x0 > w - ow || y0 > h - oh) {
-    set_error("%s: the window (%d, %d, %d, %d) leaves the %d x %d input", what, x0, y0, ow, oh, w, h);
-    return VWB200_EARG;
-  }
-  if (rasters_overlap(disparity, w, h, pitch, xyz, ow, oh, xyz_pitch, 12, 24)) { set_error("%s: xyz overlaps the disparity", what); return VWB200_EARG; }
+  VWB_TRY(triangulate_args(what, disparity, w, h, pitch, x0, y0, ow, oh, xyz, xyz_pitch));
   TriCam c0, c1;
   double tol;
   VWB_TRY(cameras_open(what, cam1, cam2, angle_tol, &c0, &c1, &tol));
@@ -1965,13 +1985,7 @@ int vwb200_stereo_model_points(const float* disparity, int w, int h, ptrdiff_t p
   if (!disparity || !xyz || !error) { set_error("%s: null disparity or output", what); return VWB200_EARG; }
   VWB_TRY(pinhole_check(what, cam1));
   VWB_TRY(pinhole_check(what, cam2));
-  if (w <= 0 || h <= 0 || pitch < w) { set_error("%s: bad input size %d x %d, pitch %td", what, w, h, pitch); return VWB200_EARG; }
-  if (xyz_pitch < w || error_pitch < w) { set_error("%s: output pitches %td, %td are below the width %d", what, xyz_pitch, error_pitch, w); return VWB200_EARG; }
-  if (rasters_overlap(disparity, w, h, pitch, xyz, w, h, xyz_pitch, 12, 24) || rasters_overlap(disparity, w, h, pitch, error, w, h, error_pitch, 12, 8) ||
-      rasters_overlap(xyz, w, h, xyz_pitch, error, w, h, error_pitch, 24, 8)) {
-    set_error("%s: the disparity, xyz and error rasters overlap", what);
-    return VWB200_EARG;
-  }
+  VWB_TRY(model_points_args(what, disparity, w, h, pitch, xyz, xyz_pitch, error, error_pitch));
   TriCam c0, c1;
   double tol;
   VWB_TRY(cameras_open(what, cam1, cam2, angle_tol, &c0, &c1, &tol));
@@ -2208,13 +2222,10 @@ int vwb200_resize_epipolar_cameras_to_fit(const vwb200_pinhole* cam1, const vwb2
   return VWB200_OK;
 }
 
-int vwb200_camera_transform(const vwb200_pinhole* src, const vwb200_pinhole* dst, int pixel_type, int interp, int edge, const float edge_value[2],
-                            const void* in, int w, int h, ptrdiff_t pitch, int x0, int y0, void* out, int ow, int oh, ptrdiff_t opitch,
-                            int on_device, void* stream) {
-  const char* what = "camera_transform";
-  if (!in || !out) { set_error("%s: null input or output", what); return VWB200_EARG; }
-  VWB_TRY(pinhole_check(what, src));
-  VWB_TRY(pinhole_check(what, dst));
+// the raster, pixel type, interpolation and edge checks of camera_transform (after the cameras'): VWB200_EARG, then
+// VWB200_ENOIMPL for the combinations without a device form
+static int camera_transform_args(const char* what, int pixel_type, int interp, int edge, const float* edge_value, const void* in, int w, int h,
+                                 ptrdiff_t pitch, int x0, int y0, const void* out, int ow, int oh, ptrdiff_t opitch) {
   if (pixel_type != VWB200_PIXEL_GRAY_F32 && pixel_type != VWB200_PIXEL_MASK_F32) { set_error("%s: unknown pixel type %d", what, pixel_type); return VWB200_EARG; }
   if (interp != VWB200_INTERP_BILINEAR && interp != VWB200_INTERP_BICUBIC && interp != VWB200_INTERP_NEAREST) {
     set_error("%s: unknown interpolation %d", what, interp);
@@ -2236,6 +2247,32 @@ int vwb200_camera_transform(const vwb200_pinhole* src, const vwb200_pinhole* dst
               masked ? "this interpolation of PixelMask<float> pixels" : "ValueEdgeExtension of float pixels");
     return VWB200_ENOIMPL;
   }
+  return VWB200_OK;
+}
+
+// camera_transform's image and window, staged: float pixels, or {value, valid} pairs staged as such
+static int camera_transform_stage(AbiCall& c, bool masked, const void* in, int w, int h, ptrdiff_t pitch, void* out, int ow, int oh, ptrdiff_t opitch,
+                                  int on_device, const float** din, ptrdiff_t* dp, float** dout, ptrdiff_t* dop) {
+  if (masked) {
+    const MaskF* mi; MaskF* mo;
+    VWB_TRY(c.in((const MaskF*)in, w, h, pitch, on_device, &mi, dp));
+    VWB_TRY(c.out((MaskF*)out, ow, oh, opitch, on_device, &mo, dop));
+    *din = (const float*)mi; *dout = (float*)mo;
+    return VWB200_OK;
+  }
+  VWB_TRY(c.in((const float*)in, w, h, pitch, on_device, din, dp));
+  return c.out((float*)out, ow, oh, opitch, on_device, dout, dop);
+}
+
+int vwb200_camera_transform(const vwb200_pinhole* src, const vwb200_pinhole* dst, int pixel_type, int interp, int edge, const float edge_value[2],
+                            const void* in, int w, int h, ptrdiff_t pitch, int x0, int y0, void* out, int ow, int oh, ptrdiff_t opitch,
+                            int on_device, void* stream) {
+  const char* what = "camera_transform";
+  if (!in || !out) { set_error("%s: null input or output", what); return VWB200_EARG; }
+  VWB_TRY(pinhole_check(what, src));
+  VWB_TRY(pinhole_check(what, dst));
+  VWB_TRY(camera_transform_args(what, pixel_type, interp, edge, edge_value, in, w, h, pitch, x0, y0, out, ow, oh, opitch));
+  const bool masked = pixel_type == VWB200_PIXEL_MASK_F32;
   const float ev[2] = {edge_value ? edge_value[0] : 0.0f, edge_value ? edge_value[1] : 0.0f};
   TriCam s, d;
   VWB_TRY(pinhole_build(what, *src, &s));
@@ -2246,15 +2283,7 @@ int vwb200_camera_transform(const vwb200_pinhole* src, const vwb200_pinhole* dst
   VWB_TRY(c.open(stream, on_device));
   const float* din; ptrdiff_t dp;
   float* dout; ptrdiff_t dop;
-  if (masked) {                                                  // {value, valid} pairs, staged as such
-    const MaskF* mi; MaskF* mo;
-    VWB_TRY(c.in((const MaskF*)in, w, h, pitch, on_device, &mi, &dp));
-    VWB_TRY(c.out((MaskF*)out, ow, oh, opitch, on_device, &mo, &dop));
-    din = (const float*)mi; dout = (float*)mo;
-  } else {
-    VWB_TRY(c.in((const float*)in, w, h, pitch, on_device, &din, &dp));
-    VWB_TRY(c.out((float*)out, ow, oh, opitch, on_device, &dout, &dop));
-  }
+  VWB_TRY(camera_transform_stage(c, masked, in, w, h, pitch, out, ow, oh, opitch, on_device, &din, &dp, &dout, &dop));
   unsigned long long* fail;
   VWB_TRY(c.ar.alloc(&fail, 2));
   const unsigned long long finit[2] = {0, ULLONG_MAX};
@@ -2268,6 +2297,296 @@ int vwb200_camera_transform(const vwb200_pinhole* src, const vwb200_pinhole* dst
 }
 
 // ---- the view -------------------------------------------------------------------------------------
+// ---- CAHV / CAHVOR cameras (Camera/CAHVModel.cc, CAHVORModel.cc, CameraTransform.h, StereoModel.cc:121-122) ---------------------
+// The host restatement of the camera math (linearize_camera calls pixel_to_vector); cahv.cuh is the device one.  x86-64 host
+// code has no FMA to contract into, so each operation rounds as the reference's does.
+static void scale3h(double s, const double* a, double* r) { for (int i = 0; i < 3; ++i) r[i] = s * a[i]; }
+static void normalize3h(const double* a, double* r) {          // Math/Vector.h:1694: each component / norm_2
+  const double n = std::sqrt(dot3h(a, a));
+  for (int i = 0; i < 3; ++i) r[i] = a[i] / n;
+}
+// dot_prod(cross_prod(V, H), A) < 0: a left-handed camera, whose rays pixel_to_vector negates
+static bool cahv_left_handed(const vwb200_cahv& c) {
+  double t[3];
+  cross3h(c.V, c.H, t);
+  return dot3h(t, c.A) < 0.0;
+}
+
+static int cahv_check(const char* what, const vwb200_cahv* c) {
+  if (!c) { set_error("%s: null camera", what); return VWB200_EARG; }
+  if (c->model != VWB200_CAMERA_CAHV && c->model != VWB200_CAMERA_CAHVOR) { set_error("%s: unknown camera model %d", what, c->model); return VWB200_EARG; }
+  return VWB200_OK;
+}
+
+static CahvCam cahv_build(const vwb200_cahv& c) {
+  CahvCam d;
+  std::memcpy(d.C, c.C, sizeof d.C); std::memcpy(d.A, c.A, sizeof d.A); std::memcpy(d.H, c.H, sizeof d.H);
+  std::memcpy(d.V, c.V, sizeof d.V); std::memcpy(d.O, c.O, sizeof d.O); std::memcpy(d.R, c.R, sizeof d.R);
+  d.cahvor = c.model == VWB200_CAMERA_CAHVOR;
+  d.flip = cahv_left_handed(c);
+  return d;
+}
+
+// CAHVORModel::pixel_to_vector(pix), the overload without partial derivatives (CAHVORModel.cc:297-348)
+static void cahvor_pixel_to_vector(const vwb200_cahv& c, double x, double y, double* out) {
+  double f[3], g[3], t[3], rr[3], lambda[3];
+  for (int i = 0; i < 3; ++i) { f[i] = c.V[i] - y * c.A[i]; g[i] = c.H[i] - x * c.A[i]; }
+  cross3h(f, g, t);
+  normalize3h(t, rr);
+  if (cahv_left_handed(c)) scale3h(-1.0, rr, rr);
+  const double omega = dot3h(rr, c.O);
+  for (int i = 0; i < 3; ++i) lambda[i] = rr[i] - omega * c.O[i];
+  const double tau = dot3h(lambda, lambda) / (omega * omega);
+  const double k1 = 1 + c.R[0], k3 = c.R[1] * tau, k5 = c.R[2] * tau * tau;
+  double u = 1.0 - (c.R[0] + k3 + k5);
+  for (int i = 0;; i++) {
+    if (i >= 20) break;                                          // VW_CAHVOR_MAXITER
+    const double u_2 = u * u;
+    const double poly = ((k5 * u_2 + k3) * u_2 + k1) * u - 1;
+    const double deriv = (5 * k5 * u_2 + 3 * k3) * u_2 + k1;
+    if (deriv <= 0) break;
+    const double du = poly / deriv;
+    u -= du;
+    if (std::fabs(du) < 1.0e-6) break;                           // VW_CAHVOR_CONV
+  }
+  for (int i = 0; i < 3; ++i) t[i] = rr[i] - (1 - u) * lambda[i];
+  normalize3h(t, out);
+}
+
+int vwb200_cahv_epipolar(const vwb200_cahv* cam0, const vwb200_cahv* cam1, vwb200_cahv* epi0, vwb200_cahv* epi1) {
+  const char* what = "epipolar";
+  if (!epi0 || !epi1) { set_error("%s: null output camera", what); return VWB200_EARG; }
+  VWB_TRY(cahv_check(what, cam0));
+  VWB_TRY(cahv_check(what, cam1));
+  if (cam0->model != VWB200_CAMERA_CAHV || cam1->model != VWB200_CAMERA_CAHV) {
+    set_error("%s: epipolar() takes CAHV cameras (linearize_camera takes a CAHVOR camera to one)", what);
+    return VWB200_EARG;
+  }
+  const vwb200_cahv& s0 = *cam0;
+  const vwb200_cahv& s1 = *cam1;
+  double t[3];
+  const double hc = dot3h(s0.H, s0.A) / 2.0 + dot3h(s1.H, s1.A) / 2.0;
+  const double vc = dot3h(s0.V, s0.A) / 2.0 + dot3h(s1.V, s1.A) / 2.0;
+  cross3h(s0.A, s0.H, t);
+  double hs = std::sqrt(dot3h(t, t)) / 2.0;
+  cross3h(s1.A, s1.H, t);
+  hs = hs + std::sqrt(dot3h(t, t)) / 2.0;
+  cross3h(s0.A, s0.V, t);
+  double vs = std::sqrt(dot3h(t, t)) / 2.0;
+  cross3h(s1.A, s1.V, t);
+  vs = vs + std::sqrt(dot3h(t, t)) / 2.0;
+  double app[3], dc[3], f[3], hp[3], g[3], a[3], vp[3];
+  for (int i = 0; i < 3; ++i) { app[i] = s0.A[i] + s1.A[i]; dc[i] = s1.C[i] - s0.C[i]; }
+  cross3h(app, dc, t);
+  cross3h(t, app, f);
+  const double nf = std::sqrt(dot3h(f, f));
+  if (dot3h(f, s0.H) > 0)
+    for (int i = 0; i < 3; ++i) hp[i] = f[i] * hs / nf;
+  else
+    for (int i = 0; i < 3; ++i) hp[i] = -f[i] * hs / nf;
+  for (int i = 0; i < 3; ++i) app[i] *= 0.5;
+  const double dh = dot3h(app, hp);
+  for (int i = 0; i < 3; ++i) { g[i] = hp[i] * dh / (hs * hs); t[i] = app[i] - g[i]; }
+  normalize3h(t, a);
+  cross3h(a, hp, t);
+  for (int i = 0; i < 3; ++i) vp[i] = t[i] * vs / hs;
+  vwb200_cahv e{};
+  e.model = VWB200_CAMERA_CAHV;
+  for (int i = 0; i < 3; ++i) { e.A[i] = a[i]; e.H[i] = hp[i] + hc * a[i]; e.V[i] = vp[i] + vc * a[i]; }
+  vwb200_cahv e1 = e;                                            // the outputs may be the inputs
+  std::memcpy(e.C, s0.C, sizeof e.C);
+  std::memcpy(e1.C, s1.C, sizeof e1.C);
+  *epi0 = e;
+  *epi1 = e1;
+  return VWB200_OK;
+}
+
+int vwb200_linearize_camera(const vwb200_cahv* cam, const int32_t cahvor_size[2], const int32_t cahv_size[2], vwb200_cahv* out) {
+  const char* what = "linearize_camera";
+  if (!cahvor_size || !cahv_size || !out) { set_error("%s: null size or output camera", what); return VWB200_EARG; }
+  VWB_TRY(cahv_check(what, cam));
+  if (cam->model != VWB200_CAMERA_CAHVOR) { set_error("%s: linearize_camera() takes a CAHVOR camera", what); return VWB200_EARG; }
+  const vwb200_cahv c = *cam;                                    // out may be cam
+  const int ix = cahvor_size[0], iy = cahvor_size[1];
+  // the landmarks around the perimeter; vpts[4] divides in int where vpts[1] divides in double, as the reference does
+  const double hpts[6][2] = {{0, 0}, {0, (iy - 1) / 2.0}, {0, (double)(iy - 1)}, {(double)(ix - 1), 0}, {(double)(ix - 1), (iy - 1) / 2.0},
+                             {ix - 1.0, iy - 1.0}};
+  const double vpts[6][2] = {{0, 0}, {(ix - 1) / 2.0, 0}, {(double)(ix - 1), 0}, {0, (double)(iy - 1)}, {(double)((ix - 1) / 2), (double)(iy - 1)},
+                             {ix - 1.0, iy - 1.0}};
+  double A[3] = {0.0, 0.0, 0.0}, r[3];
+  for (int k = 0; k < 6; ++k) { cahvor_pixel_to_vector(c, vpts[k][0], vpts[k][1], r); for (int i = 0; i < 3; ++i) A[i] += r[i]; }
+  for (int k = 0; k < 6; ++k) { cahvor_pixel_to_vector(c, hpts[k][0], hpts[k][1], r); for (int i = 0; i < 3; ++i) A[i] += r[i]; }
+  normalize3h(A, A);
+  double dn[3], rt[3], t[3];
+  cross3h(c.A, c.H, dn);
+  cross3h(dn, c.A, t);
+  normalize3h(t, rt);
+  normalize3h(dn, dn);
+  cross3h(dn, A, rt);
+  cross3h(A, rt, t);
+  normalize3h(t, dn);
+  normalize3h(rt, rt);
+  double hmin = 1, hmax = -1, vmin = 1, vmax = -1;
+  for (int k = 0; k < 6; ++k) {
+    double u3[3], w3[3];
+    cahvor_pixel_to_vector(c, hpts[k][0], hpts[k][1], u3);
+    const double d = dot3h(dn, u3);
+    for (int i = 0; i < 3; ++i) t[i] = u3[i] - d * dn[i];
+    normalize3h(t, w3);
+    cross3h(A, w3, t);
+    const double sn = std::sqrt(dot3h(t, t));
+    if (hmin > sn) hmin = sn;
+    if (hmax < sn) hmax = sn;
+  }
+  for (int k = 0; k < 6; ++k) {
+    double u3[3], w3[3];
+    cahvor_pixel_to_vector(c, vpts[k][0], vpts[k][1], u3);
+    const double d = dot3h(rt, u3);
+    for (int i = 0; i < 3; ++i) t[i] = u3[i] - d * rt[i];
+    normalize3h(t, w3);
+    cross3h(A, w3, t);
+    const double sn = std::sqrt(dot3h(t, t));
+    if (vmin > sn) vmin = sn;
+    if (vmax < sn) vmax = sn;
+  }
+  // minfov: the smaller field of view
+  const double ic[2] = {((double)cahv_size[0] - 1.0) / 2.0, ((double)cahv_size[1] - 1.0) / 2.0};
+  const double ic2[2] = {ic[0] * ic[0], ic[1] * ic[1]};
+  const double sf[2] = {std::sqrt(ic2[0] / (hmin * hmin) - ic2[0]), std::sqrt(ic2[1] / (vmin * vmin) - ic2[1])};
+  vwb200_cahv o{};
+  o.model = VWB200_CAMERA_CAHV;
+  for (int i = 0; i < 3; ++i) {
+    o.C[i] = c.C[i];
+    o.A[i] = A[i];
+    o.H[i] = sf[0] * rt[i] + ic[0] * A[i];
+    o.V[i] = sf[1] * dn[i] + ic[1] * A[i];
+  }
+  *out = o;
+  return VWB200_OK;
+}
+
+int vwb200_pinhole_to_cahv(const vwb200_pinhole* pin, vwb200_cahv* out) {
+  const char* what = "CAHVModel = PinholeModel";
+  if (!out) { set_error("%s: null output camera", what); return VWB200_EARG; }
+  VWB_TRY(pinhole_check(what, pin));
+  if (pin->lens != VWB200_LENS_NULL) { set_error("%s: the pinhole has a lens distortion, which a CAHV camera cannot carry", what); return VWB200_EARG; }
+  TriCam t;
+  VWB_TRY(pinhole_build(what, *pin, &t));                        // a camera the reference can construct
+  const double pitch = pin->pixel_pitch;
+  if (pitch == 0) { set_error("%s: CAHVModel::operator=() input pinhole model has zero pitch!", what); return VWB200_EARG; }
+  const double fH = pin->fu / pitch, fV = pin->fv / pitch, cH = pin->cu / pitch, cV = pin->cv / pitch;
+  double Hv[3], Vv[3], A[3];
+  for (int i = 0; i < 3; ++i) {                                  // R * u, R * v, R * w: row i of R . the vector, from 0.0
+    Hv[i] = dot3h(pin->rotation + 3 * i, pin->u_direction);
+    Vv[i] = dot3h(pin->rotation + 3 * i, pin->v_direction);
+    A[i] = dot3h(pin->rotation + 3 * i, pin->w_direction);
+  }
+  vwb200_cahv o{};
+  o.model = VWB200_CAMERA_CAHV;
+  for (int i = 0; i < 3; ++i) {
+    o.C[i] = pin->center[i];
+    o.A[i] = A[i];
+    o.H[i] = fH * Hv[i] + cH * A[i];
+    o.V[i] = fV * Vv[i] + cV * A[i];
+  }
+  *out = o;
+  return VWB200_OK;
+}
+
+int vwb200_cahv_camera_transform(const vwb200_cahv* src, const vwb200_cahv* dst, int pixel_type, int interp, int edge, const float edge_value[2],
+                                 const void* in, int w, int h, ptrdiff_t pitch, int x0, int y0, void* out, int ow, int oh, ptrdiff_t opitch,
+                                 int on_device, void* stream) {
+  const char* what = "camera_transform";
+  if (!in || !out) { set_error("%s: null input or output", what); return VWB200_EARG; }
+  VWB_TRY(cahv_check(what, src));
+  VWB_TRY(cahv_check(what, dst));
+  VWB_TRY(camera_transform_args(what, pixel_type, interp, edge, edge_value, in, w, h, pitch, x0, y0, out, ow, oh, opitch));
+  if (dst->model != VWB200_CAMERA_CAHV) { set_error("%s: the destination camera must be CAHV (a CAHVOR one has no device form)", what); return VWB200_ENOIMPL; }
+  if (!(src->C[0] == dst->C[0] && src->C[1] == dst->C[1] && src->C[2] == dst->C[2])) {
+    set_error("%s: CameraTransformFunctor: Camera transformation require that the camera center is always the same for both cameras.", what);
+    return VWB200_ELOGIC;
+  }
+  const bool masked = pixel_type == VWB200_PIXEL_MASK_F32;
+  const float ev[2] = {edge_value ? edge_value[0] : 0.0f, edge_value ? edge_value[1] : 0.0f};
+  const CahvCam s = cahv_build(*src), d = cahv_build(*dst);
+  VWB_TRY(ensure_device());
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
+  const float* din; ptrdiff_t dp;
+  float* dout; ptrdiff_t dop;
+  VWB_TRY(camera_transform_stage(c, masked, in, w, h, pitch, out, ow, oh, opitch, on_device, &din, &dp, &dout, &dop));
+  VWB_TRY(cahv_warp_launch(masked, interp, edge, ev, s, d, din, w, h, dp, x0, y0, dout, ow, oh, dop, c.st));
+  return c.finish();
+}
+
+int vwb200_cahv_stereo_triangulate(int pixel_type, const void* disparity, int w, int h, ptrdiff_t pitch, int x0, int y0, int ow, int oh,
+                                   const vwb200_cahv* cam1, const vwb200_cahv* cam2, double angle_tol, double* xyz, ptrdiff_t xyz_pitch,
+                                   int on_device, void* stream) {
+  t_tri_stats = vwb200_triangulation_stats{0, 0, 0.0, 0.0, 0, 0};
+  const char* what = "stereo_triangulate";
+  if (!disparity || !xyz) { set_error("%s: null disparity or output", what); return VWB200_EARG; }
+  if (pixel_type != VWB200_DISP_I32 && pixel_type != VWB200_DISP_F32) { set_error("%s: unknown pixel type %d", what, pixel_type); return VWB200_EARG; }
+  VWB_TRY(cahv_check(what, cam1));
+  VWB_TRY(cahv_check(what, cam2));
+  VWB_TRY(triangulate_args(what, disparity, w, h, pitch, x0, y0, ow, oh, xyz, xyz_pitch));
+  const CahvCam c0 = cahv_build(*cam1), c1 = cahv_build(*cam2);
+  const double tol = angle_tol > 0 ? angle_tol : 1e-4;
+  VWB_TRY(ensure_device());
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
+  Pt3* dxyz; ptrdiff_t dxp;
+  VWB_TRY(c.out((Pt3*)xyz, ow, oh, xyz_pitch, on_device, &dxyz, &dxp));
+  unsigned long long* dst;
+  VWB_TRY(tri_stats_open(c, &dst, 6));
+  if (pixel_type == VWB200_DISP_I32) {
+    const vwb200_dispi* din; ptrdiff_t dp;
+    VWB_TRY(c.in((const vwb200_dispi*)disparity + (ptrdiff_t)y0 * pitch + x0, ow, oh, pitch, on_device, &din, &dp));
+    VWB_TRY(cahv_stereo_triangulate_launch(din, dp, x0, y0, ow, oh, c0, c1, tol, (double*)dxyz, dxp, dst, c.st));
+  } else {
+    const DispF* din; ptrdiff_t dp;
+    VWB_TRY(c.in((const DispF*)disparity + (ptrdiff_t)y0 * pitch + x0, ow, oh, pitch, on_device, &din, &dp));
+    VWB_TRY(cahv_stereo_triangulate_launch(din, dp, x0, y0, ow, oh, c0, c1, tol, (double*)dxyz, dxp, dst, c.st));
+  }
+  unsigned long long s[6];
+  VWB_CUDA(cudaMemcpyAsync(s, dst, sizeof s, cudaMemcpyDeviceToHost, c.st));
+  VWB_TRY(c.finish());
+  t_tri_stats.cahvor_iterations = (long long)s[5];
+  return VWB200_OK;
+}
+
+int vwb200_cahv_stereo_model_points(const float* disparity, int w, int h, ptrdiff_t pitch, const vwb200_cahv* cam1, const vwb200_cahv* cam2,
+                                    double angle_tol, double* xyz, ptrdiff_t xyz_pitch, double* error, ptrdiff_t error_pitch, int on_device,
+                                    void* stream) {
+  t_tri_stats = vwb200_triangulation_stats{0, 0, 0.0, 0.0, 0, 0};
+  const char* what = "StereoModel";
+  if (!disparity || !xyz || !error) { set_error("%s: null disparity or output", what); return VWB200_EARG; }
+  VWB_TRY(cahv_check(what, cam1));
+  VWB_TRY(cahv_check(what, cam2));
+  VWB_TRY(model_points_args(what, disparity, w, h, pitch, xyz, xyz_pitch, error, error_pitch));
+  const CahvCam c0 = cahv_build(*cam1), c1 = cahv_build(*cam2);
+  const double tol = angle_tol > 0 ? angle_tol : 1e-4;
+  VWB_TRY(ensure_device());
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
+  const DispF* din; ptrdiff_t dp;
+  VWB_TRY(c.in((const DispF*)disparity, w, h, pitch, on_device, &din, &dp));
+  Pt3* dxyz; ptrdiff_t dxp;
+  VWB_TRY(c.out((Pt3*)xyz, w, h, xyz_pitch, on_device, &dxyz, &dxp));
+  double* derr; ptrdiff_t dep;
+  VWB_TRY(c.out(error, w, h, error_pitch, on_device, &derr, &dep));
+  unsigned long long* dst;
+  VWB_TRY(tri_stats_open(c, &dst, 6));
+  VWB_TRY(cahv_stereo_model_launch(din, w, h, dp, c0, c1, tol, (double*)dxyz, dxp, derr, dep, dst, c.st));
+  unsigned long long s[6];
+  VWB_CUDA(cudaMemcpyAsync(s, dst, sizeof s, cudaMemcpyDeviceToHost, c.st));
+  VWB_TRY(c.finish());
+  double sum, mx;
+  std::memcpy(&sum, &s[0], sizeof sum);
+  std::memcpy(&mx, &s[1], sizeof mx);
+  t_tri_stats = vwb200_triangulation_stats{(long long)s[2], (long long)s[3], mx, sum, 0, (long long)s[5]};
+  return VWB200_OK;
+}
+
 int vwb200_corr_create(const vwb200_corr_params* p, vwb200_corr** out) {
   if (!p || !out) { set_error("corr_create: null pointer"); return VWB200_EARG; }
   const double w = (double)p->search_x1 - p->search_x0, h = (double)p->search_y1 - p->search_y0;

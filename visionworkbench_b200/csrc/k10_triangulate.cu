@@ -5,7 +5,8 @@
 // One thread per pixel, grid-stride over rows.  Each warp stages its 32 {x, y, z} results in shared memory and stores them as
 // three contiguous 256-byte runs.  The cameras are kernel parameters (TriCam: the inverse camera transform the host builds
 // once per call, the center, the pixel pitch and the lens); the camera math is pinhole.cuh's, bit for bit the reference's.
-#include "pinhole.cuh"
+// k10_triangulate_cahv_kernel<T, MODEL> is the same pass through CAHV / CAHVOR cameras (cahv.cuh): only the rays differ.
+#include "cahv.cuh"
 
 namespace vwb200 {
 namespace {
@@ -13,17 +14,10 @@ namespace {
 constexpr int kThreads = 128;                  // pixels of one row per CTA
 constexpr int kWarps = kThreads / 32;
 
-// StereoModel::operator()(pix1, pix2, errorVec) for two cameras (StereoModel.cc:35-48, 68-91, 97-147)
-template <bool TSAI>
-__device__ __forceinline__ V3 triangulate(const TriCam& c0, const TriCam& c1, double tol, double l0, double l1, double r0, double r1,
-                                          V3* err, int* iters) {
-  *err = V3{0.0, 0.0, 0.0};
-  const bool ok0 = !(l0 != l0 || l1 != l1) && !(l0 == -1e8 && l1 == -1e8);     // NaN or invalid_pixel(): the ray is skipped
-  const bool ok1 = !(r0 != r0 || r1 != r1) && !(r0 == -1e8 && r1 == -1e8);
-  if (!ok0 || !ok1) return V3{0.0, 0.0, 0.0};
-  const V3 d0 = pixel_to_vector<TSAI>(c0, l0, l1, iters), d1 = pixel_to_vector<TSAI>(c1, r0, r1, iters);
+// the rays' part of StereoModel::operator()(pix1, pix2, errorVec) (StereoModel.cc:35-48, 68-91, 97-147): the nearly-parallel
+// test, triangulate_pair and the reflection through C0; *err is zero on entry
+__device__ __forceinline__ V3 intersect(const V3 C0, const V3 C1, const V3 d0, const V3 d1, double tol, V3* err) {
   if (!(dsub(1.0, dot3(d0, d1)) >= tol)) return V3{0.0, 0.0, 0.0};              // nearly parallel (NaN counts as parallel)
-  const V3 C0{c0.c[0], c0.c[1], c0.c[2]}, C1{c1.c[0], c1.c[1], c1.c[2]};
   const V3 v12 = cross3(d0, d1), v1 = cross3(v12, d0), v2 = cross3(v12, d1);
   const double s1 = ddiv(dot3(v2, sub3(C1, C0)), dot3(v2, d0));
   const double s2 = ddiv(dot3(v1, sub3(C0, C1)), dot3(v1, d1));
@@ -34,6 +28,29 @@ __device__ __forceinline__ V3 triangulate(const TriCam& c0, const TriCam& c1, do
   if (dot3(sub3(r, C0), d0) < 0 || dot3(sub3(r, C1), d1) < 0)                    // behind a camera: reflect through C0
     r = V3{dadd(-r.x, dmul(2.0, C0.x)), dadd(-r.y, dmul(2.0, C0.y)), dadd(-r.z, dmul(2.0, C0.z))};
   return r;
+}
+
+// StereoModel::operator()(pix1, pix2, errorVec) for two pinhole cameras
+template <bool TSAI>
+__device__ __forceinline__ V3 triangulate(const TriCam& c0, const TriCam& c1, double tol, double l0, double l1, double r0, double r1,
+                                          V3* err, int* iters) {
+  *err = V3{0.0, 0.0, 0.0};
+  const bool ok0 = !(l0 != l0 || l1 != l1) && !(l0 == -1e8 && l1 == -1e8);     // NaN or invalid_pixel(): the ray is skipped
+  const bool ok1 = !(r0 != r0 || r1 != r1) && !(r0 == -1e8 && r1 == -1e8);
+  if (!ok0 || !ok1) return V3{0.0, 0.0, 0.0};
+  const V3 d0 = pixel_to_vector<TSAI>(c0, l0, l1, iters), d1 = pixel_to_vector<TSAI>(c1, r0, r1, iters);
+  return intersect(V3{c0.c[0], c0.c[1], c0.c[2]}, V3{c1.c[0], c1.c[1], c1.c[2]}, d0, d1, tol, err);
+}
+
+// the same through CAHV / CAHVOR cameras (StereoModel.cc:121-122 takes any camera's pixel_to_vector and camera_center)
+__device__ __forceinline__ V3 triangulate_cahv(const CahvCam& c0, const CahvCam& c1, double tol, double l0, double l1, double r0, double r1,
+                                               V3* err, int* iters) {
+  *err = V3{0.0, 0.0, 0.0};
+  const bool ok0 = !(l0 != l0 || l1 != l1) && !(l0 == -1e8 && l1 == -1e8);
+  const bool ok1 = !(r0 != r0 || r1 != r1) && !(r0 == -1e8 && r1 == -1e8);
+  if (!ok0 || !ok1) return V3{0.0, 0.0, 0.0};
+  const V3 d0 = cahv_pixel_to_vector<true>(c0, l0, l1, iters), d1 = cahv_pixel_to_vector<true>(c1, r0, r1, iters);
+  return intersect(ld3(c0.C), ld3(c1.C), d0, d1, tol, err);
 }
 
 // the 32 {x, y, z} of a warp's consecutive pixels [0, n) to row + 3 * first, as three contiguous runs
@@ -113,6 +130,52 @@ __global__ void __launch_bounds__(kThreads, 4) k10_triangulate_kernel(const T* _
   if (MODEL || TSAI) flush_stats(stats, sum, mx, pts, div, (unsigned long long)iters);
 }
 
+// a warp's sum of n added to *count
+__device__ __forceinline__ void flush_count(unsigned long long* count, unsigned long long n) {
+  for (int o = 16; o; o >>= 1) n += __shfl_xor_sync(0xffffffffu, n, o);
+  if ((threadIdx.x & 31) == 0 && n) atomicAdd(count, n);
+}
+
+// k10_triangulate_kernel's two forms through CAHV / CAHVOR cameras; stats[5] counts the CAHVOR Newton passes
+template <class T, bool MODEL>
+__global__ void __launch_bounds__(kThreads, 4) k10_triangulate_cahv_kernel(const T* __restrict__ in, ptrdiff_t ip, int x0, int y0, int ow, int oh,
+                                                                        const CahvCam c0, const CahvCam c1, double tol, double* __restrict__ xyz,
+                                                                        ptrdiff_t xp, double* __restrict__ err, ptrdiff_t ep,
+                                                                        unsigned long long* stats) {
+  __shared__ double stage[kWarps][96];
+  const int first = blockIdx.x * kThreads + (threadIdx.x & ~31);
+  const int n = min(32, ow - first);
+  const int i = blockIdx.x * kThreads + threadIdx.x;
+  double sum = 0.0, mx = 0.0;
+  unsigned long long pts = 0, div = 0;
+  int iters = 0;
+  if (n > 0) {
+    for (int j = blockIdx.y; j < oh; j += gridDim.y) {
+      V3 p{0.0, 0.0, 0.0}, e{0.0, 0.0, 0.0};
+      double error = 0.0;
+      if (i < ow) {
+        const T d = in[(ptrdiff_t)j * ip + i];
+        if (valid(d)) {
+          const int x = x0 + i, y = y0 + j;
+          if constexpr (MODEL) {
+            p = triangulate_cahv(c0, c1, tol, (double)x, (double)y, (double)__fadd_rn((float)x, chan(d, 0)), (double)__fadd_rn((float)y, chan(d, 1)),
+                                 &e, &iters);
+            error = norm3(e);
+            if (error >= 0) { mx = fmax(mx, error); sum = dadd(sum, error); ++pts; }
+            else { p = V3{0.0, 0.0, 0.0}; ++div; }
+          } else {
+            p = triangulate_cahv(c0, c1, tol, (double)x, (double)y, dadd((double)x, wide(d, 0)), dadd((double)y, wide(d, 1)), &e, &iters);
+          }
+        }
+        if constexpr (MODEL) err[(ptrdiff_t)j * ep + i] = error;
+      }
+      store_xyz(stage[threadIdx.x >> 5], xyz + (ptrdiff_t)j * xp * 3 + 3 * (ptrdiff_t)first, n, p);
+    }
+  }
+  if (MODEL) flush_stats(stats, sum, mx, pts, div, 0);
+  flush_count(stats + 5, (unsigned long long)iters);
+}
+
 // UniverseRadiusFunc::operator()(Vector3) (StereoView.h:172-186) over a w x h Vector3 image; in may be out (same pitch).
 // stats[0] counts the rejected points.
 __global__ void __launch_bounds__(kThreads) k10_universe_radius_kernel(const double* in, ptrdiff_t ip, int w, int h, V3 o, double nr,
@@ -177,6 +240,25 @@ int stereo_model_launch(const DispF* in, int w, int h, ptrdiff_t ip, const TriCa
     k10_triangulate_kernel<DispF, true, true><<<g, kThreads, 0, st>>>(in, ip, 0, 0, w, h, c0, c1, tol, xyz, xp, err, ep, stats);
   else
     k10_triangulate_kernel<DispF, true, false><<<g, kThreads, 0, st>>>(in, ip, 0, 0, w, h, c0, c1, tol, xyz, xp, err, ep, stats);
+  VWB_LAUNCH_CHECK();
+  return VWB200_OK;
+}
+
+template <class T>
+int cahv_stereo_triangulate_launch(const T* in, ptrdiff_t ip, int x0, int y0, int ow, int oh, const CahvCam& c0, const CahvCam& c1, double tol,
+                                   double* xyz, ptrdiff_t xp, unsigned long long* stats, cudaStream_t st) {
+  k10_triangulate_cahv_kernel<T, false><<<grid_for(ow, oh), kThreads, 0, st>>>(in, ip, x0, y0, ow, oh, c0, c1, tol, xyz, xp, nullptr, 0, stats);
+  VWB_LAUNCH_CHECK();
+  return VWB200_OK;
+}
+template int cahv_stereo_triangulate_launch<vwb200_dispi>(const vwb200_dispi*, ptrdiff_t, int, int, int, int, const CahvCam&, const CahvCam&,
+                                                          double, double*, ptrdiff_t, unsigned long long*, cudaStream_t);
+template int cahv_stereo_triangulate_launch<DispF>(const DispF*, ptrdiff_t, int, int, int, int, const CahvCam&, const CahvCam&, double, double*,
+                                                   ptrdiff_t, unsigned long long*, cudaStream_t);
+
+int cahv_stereo_model_launch(const DispF* in, int w, int h, ptrdiff_t ip, const CahvCam& c0, const CahvCam& c1, double tol, double* xyz,
+                             ptrdiff_t xp, double* err, ptrdiff_t ep, unsigned long long* stats, cudaStream_t st) {
+  k10_triangulate_cahv_kernel<DispF, true><<<grid_for(w, h), kThreads, 0, st>>>(in, ip, 0, 0, w, h, c0, c1, tol, xyz, xp, err, ep, stats);
   VWB_LAUNCH_CHECK();
   return VWB200_OK;
 }

@@ -8,8 +8,10 @@
 // The internal kinds kCamera (float pixels) and kCameraMasked (PixelMask<float>, bilinear) are CameraTransform(src, dst)
 // (Camera/CameraTransform.h:52-61) between pinhole cameras, through pinhole.cuh: reverse(p) = src.point_to_pixel(
 // dst.pixel_to_vector(p) + C), with point_to_pixel's check.  k8_camera_bbox_kernel is the bbox pass of
-// resize_epipolar_cameras_to_fit through the same cameras.
-#include "pinhole.cuh"
+// resize_epipolar_cameras_to_fit through the same cameras.  The internal kinds kCahv and kCahvMasked are the same transform
+// from a CAHV or CAHVOR src into a CAHV dst, through cahv.cuh (the src model is a runtime branch on its flag; the dst is CAHV
+// at compile time, so the CAHVOR Newton loop is not compiled in; the CAHV family has no point_to_pixel check).
+#include "cahv.cuh"
 
 namespace vwb200 {
 namespace {
@@ -20,6 +22,8 @@ constexpr int kTW = 32, kTH = 8;
 constexpr double kDomain = 1073741824.0;               // 2^30
 constexpr int kCamera = 2;                             // beside VWB200_WARP_HOMOGRAPHY and VWB200_WARP_DISPARITY
 constexpr int kCameraMasked = 3;                       // kCamera over PixelMask<float> {value, valid} pixels
+constexpr int kCahv = 4;                               // kCamera through CAHV / CAHVOR cameras
+constexpr int kCahvMasked = 5;                         // kCameraMasked through CAHV / CAHVOR cameras
 
 // math::impl::_floor and _round for double -> int32 (Math/Functions.h:48-51, 74-81)
 __device__ __forceinline__ int vw_floor(double v) {
@@ -133,7 +137,8 @@ struct WarpArgs {
   float* out; int ow, oh; ptrdiff_t op;
   TriCam src, dst;                                     // kCamera only (appended: the other kinds' parameters keep their offsets)
   unsigned long long* fail;                            // kCamera: {any check failed, first failing row-major window index}
-  float2 ev;                                           // kCameraMasked: the VWB200_EDGE_VALUE pixel {value, valid}
+  float2 ev;                                           // kCameraMasked, kCahvMasked: the VWB200_EDGE_VALUE pixel {value, valid}
+  CahvCam csrc, cdst;                                  // kCahv, kCahvMasked only (appended, as src and dst were)
 };
 
 // one thread per output pixel of a 32 x 8 tile; window pixel (ox, oy) is TransformView pixel (x0 + ox, y0 + oy)
@@ -159,6 +164,8 @@ __global__ void __launch_bounds__(kTW * kTH) k8_warp_kernel(const WarpArgs a) {
         a.fail[0] = 1;
         atomicMin(a.fail + 1, (unsigned long long)oy * a.ow + ox);
       }
+    } else if (Kind == kCahv || Kind == kCahvMasked) {
+      cahv_camera_map(a.cdst, a.csrc, px, py, &rx, &ry);
     } else {
       // DisparityTransform::reverse: the offset read with nearest-pixel interpolation and zero extension at the integer p
       const int ix = a.x0 + ox;
@@ -168,7 +175,7 @@ __global__ void __launch_bounds__(kTW * kTH) k8_warp_kernel(const WarpArgs a) {
         if (__ldg(d + 2) != 0.0f) { rx = __dadd_rn(px, (double)__ldg(d)); ry = __dadd_rn(py, (double)__ldg(d + 1)); }
       }
     }
-    if (Kind == kCameraMasked) {
+    if (Kind == kCameraMasked || Kind == kCahvMasked) {
       Px2 v{0.0f, 0.0f};                               // outside the domain: {0, 0}
       if (fabs(rx) < kDomain && fabs(ry) < kDomain) v = bilinear2<Edge>(a.in, a.w, a.h, a.ip, a.ev, rx, ry);
       float* q = a.out + 2 * ((ptrdiff_t)oy * a.op + ox);
@@ -238,6 +245,16 @@ int camera_warp_launch(int masked, int interp, int edge, const float* edge_value
   return launch<kCameraMasked, VWB200_INTERP_BILINEAR, VWB200_EDGE_VALUE>(a, st);
 }
 
+int cahv_warp_launch(int masked, int interp, int edge, const float* edge_value, const CahvCam& src, const CahvCam& dst, const float* in, int w,
+                     int h, ptrdiff_t ip, int x0, int y0, float* out, int ow, int oh, ptrdiff_t op, cudaStream_t st) {
+  if (ow <= 0 || oh <= 0) return VWB200_OK;
+  WarpArgs a{in, w, h, ip, nullptr, 0, 0, 0, {}, x0, y0, out, ow, oh, op, {}, {}, nullptr, make_float2(edge_value[0], edge_value[1]), src, dst};
+  if (!masked) return launch_interp<kCahv>(interp, edge, a, st);
+  if (edge == VWB200_EDGE_ZERO) return launch<kCahvMasked, VWB200_INTERP_BILINEAR, VWB200_EDGE_ZERO>(a, st);
+  if (edge == VWB200_EDGE_CONSTANT) return launch<kCahvMasked, VWB200_INTERP_BILINEAR, VWB200_EDGE_CONSTANT>(a, st);
+  return launch<kCahvMasked, VWB200_INTERP_BILINEAR, VWB200_EDGE_VALUE>(a, st);
+}
+
 int camera_bbox_launch(const TriCam& src, const TriCam& dst, int x0, int y0, int x1, int y1, unsigned* keys4, unsigned long long* fail,
                        cudaStream_t st) {
   const long long n = 2 * ((long long)x1 - x0 + (long long)y1 - y0);
@@ -250,7 +267,7 @@ int camera_bbox_launch(const TriCam& src, const TriCam& dst, int x0, int y0, int
 int warp_launch(const vwb200_warp_params& p, const float* in, int w, int h, ptrdiff_t ip, const DispF* disp, int dw, int dh, ptrdiff_t dp,
                 int x0, int y0, float* out, int ow, int oh, ptrdiff_t op, cudaStream_t st) {
   if (ow <= 0 || oh <= 0) return VWB200_OK;
-  WarpArgs a{in, w, h, ip, disp, dw, dh, dp, {}, x0, y0, out, ow, oh, op, {}, {}, nullptr, {}};
+  WarpArgs a{in, w, h, ip, disp, dw, dh, dp, {}, x0, y0, out, ow, oh, op, {}, {}, nullptr, {}, {}, {}};
   for (int i = 0; i < 9; ++i) a.m[i] = p.matrix[i];
   if (p.kind == VWB200_WARP_HOMOGRAPHY) return launch_interp<VWB200_WARP_HOMOGRAPHY>(p.interp, p.edge, a, st);
   return launch_interp<VWB200_WARP_DISPARITY>(p.interp, p.edge, a, st);
