@@ -187,7 +187,8 @@ def test_stereo_triangulate(vwb, w, h):
                 ref, it = oc.stereo_triangulate(d, c0, c1, x0, y0, ow, oh)
                 got = vwb.stereo_triangulate(d, api(vwb, c0), api(vwb, c1), bbox=(x0, y0, x0 + ow, y0 + oh))
                 assert same(got, ref), (kind, win)
-                assert vwb.last_triangulation_stats()["cahvor_iterations"] == it
+                s = vwb.last_triangulation_stats()
+                assert s["cahvor_iterations"] == it and s["tsai_iterations"] == 0, (kind, win, s)
             got = vwb.stereo_triangulate(torch.from_numpy(d).cuda(), api(vwb, c0), api(vwb, c1), angle_tol=1e-3).cpu().numpy()
             assert same(got, oc.stereo_triangulate(d, c0, c1, angle_tol=1e-3)[0])
 
@@ -201,7 +202,7 @@ def test_stereo_model_points(vwb, w, h):
         assert same(gx, xyz) and same(ge, err)
         s = vwb.last_triangulation_stats()
         assert (s["points"], s["divergent"], s["max_error"], s["cahvor_iterations"]) == (st[0], st[1], st[2], it)
-        assert abs(s["error_sum"] - st[3]) <= 1e-12 * max(1.0, abs(st[3]))
+        assert abs(s["error_sum"] - st[3]) <= 1e-12 * max(1.0, abs(st[3])) and s["tsai_iterations"] == 0
 
 
 TRACE_SCRIPT = """
@@ -242,9 +243,9 @@ for m, i, e, fn in cases:
 """
 
 
-def test_kernel_trace():
+def test_kernel_trace_per_camera_type():
     """each CAHV call ran only its own instantiation: k8_warp_kernel<4, interp, edge> / <5, 0, edge>, and
-    k10_triangulate_cahv_kernel<T, MODEL>"""
+    k10_triangulate_kernel<CahvCam, T, MODEL, true>"""
     import re
     here = os.path.dirname(os.path.abspath(__file__))
     env = dict(os.environ, PYTHONPATH=os.pathsep.join([os.path.dirname(here), here]), PYTHONNOUSERSITE="1")
@@ -262,7 +263,9 @@ def test_kernel_trace():
         else:
             t = {"ti": "vwb200_dispi", "tf": "DispF", "tm": "DispF"}[m]
             model = "true" if m == "tm" else "false"
-            assert "k10_triangulate_cahv_kernel<" in name and t in name and model in name, (m, name)
+            assert "k10_triangulate_kernel<" in name, (m, name)
+            args = name.split("<", 1)[1].split(">")[0].replace("(bool)1", "true").replace("(bool)0", "false").split(", ")
+            assert args[0].endswith("CahvCam") and args[1].endswith(t) and args[2:] == [model, "true"], (m, name)
 
 
 # ---- end to end ------------------------------------------------------------------------------------------------------------

@@ -58,6 +58,8 @@ def check_b(vwb, d, cams, angle_tol=0.0, devs=(False, True), label=""):
         s = vwb.last_triangulation_stats()
         assert (s["points"], s["divergent"], s["max_error"]) == (st["points"], st["divergent"], st["max_error"]), (s, st)
         assert abs(s["error_sum"] - st["error_sum"]) <= 1e-12 * abs(st["error_sum"]), (s, st)
+        tsai = any(c.get("tsai") is not None for c in cams) and st["points"] + st["divergent"] > 0
+        assert (s["tsai_iterations"] > 0) == tsai and s["cahvor_iterations"] == 0, (s, label)
     return xyz, err, st
 
 
@@ -155,6 +157,7 @@ def test_4096(vwb):
     s = vwb.last_triangulation_stats()
     assert (s["points"], s["divergent"], s["max_error"]) == (st["points"], st["divergent"], st["max_error"]), (s, st)
     assert abs(s["error_sum"] - st["error_sum"]) <= 1e-12 * abs(st["error_sum"]), (s, st)
+    assert s["tsai_iterations"] > 0 and s["cahvor_iterations"] == 0, s
     got = vwb.stereo_triangulate(x, api_cam(vwb, cams[0]), api_cam(vwb, cams[1]), (1000, 1500, 2024, 2524)).cpu().numpy()
     assert same(got, ot.stereo_triangulate(d, cams[0], cams[1], (1000, 1500, 1024, 1024)))
     pts = torch.from_numpy(xyz).cuda()
@@ -305,8 +308,8 @@ print("CASE", "-", "float64", "c", "|".join(sorted(set(tr.raw))))
 """
 
 
-def test_kernel_trace():
-    """each form and lens runs its own k10_triangulate_kernel<T, MODEL, TSAI> instantiation; universe radius its kernel"""
+def test_kernel_trace_per_camera_type():
+    """each form and lens runs its own k10_triangulate_kernel<TriCam, T, MODEL, TSAI> instantiation; universe radius its kernel"""
     here = os.path.dirname(os.path.abspath(__file__))
     env = dict(os.environ, PYTHONPATH=os.pathsep.join([os.path.dirname(here), here]), PYTHONNOUSERSITE="1")
     r = subprocess.run([sys.executable, "-c", TRACE_SCRIPT], cwd=here, env=env, capture_output=True, text=True, timeout=600)
@@ -322,5 +325,5 @@ def test_kernel_trace():
             continue
         assert "k10_triangulate_kernel" in name, name
         args = name.split("<", 1)[1].split(">")[0].replace("(bool)1", "true").replace("(bool)0", "false").split(", ")
-        assert args[0].endswith("vwb200_dispi" if dt == "int32" else "DispF"), name
-        assert args[1:] == ["true" if form == "b" else "false", "true" if lens == "tsai" else "false"], name
+        assert args[0].endswith("TriCam") and args[1].endswith("vwb200_dispi" if dt == "int32" else "DispF"), name
+        assert args[2:] == ["true" if form == "b" else "false", "true" if lens == "tsai" else "false"], name

@@ -761,14 +761,10 @@ def stereo_triangulate(disparity, cam1, cam2, bbox=None, angle_tol=0.0):
     t, ptr, cols, rows, pitch, dev, dt = _disparity_in(disparity)
     x0, y0, x1, y1 = _bbox(bbox) if bbox is not None else (0, 0, cols, rows)
     out = _output(t, (max(y1 - y0, 0), max(x1 - x0, 0), 3), np.float64)
-    if _family("stereo_triangulate", cam1, cam2) == "cahv":
-        _check(lib().vwb200_cahv_stereo_triangulate(_ptype(dt), ptr, cols, rows, pitch, x0, y0, x1 - x0, y1 - y0, C.byref(cam1._struct()),
-                                                    C.byref(cam2._struct()), float(angle_tol), _ptr(out), x1 - x0, dev,
-                                                    _stream_ptr() if dev else None))
-        return out
+    fn = lib().vwb200_cahv_stereo_triangulate if _family("stereo_triangulate", cam1, cam2) == "cahv" else lib().vwb200_stereo_triangulate
     c1, c2 = cam1._struct(), cam2._struct()
-    _check(lib().vwb200_stereo_triangulate(_ptype(dt), ptr, cols, rows, pitch, x0, y0, x1 - x0, y1 - y0, C.byref(c1), C.byref(c2),
-                                           float(angle_tol), _ptr(out), x1 - x0, dev, _stream_ptr() if dev else None))
+    _check(fn(_ptype(dt), ptr, cols, rows, pitch, x0, y0, x1 - x0, y1 - y0, C.byref(c1), C.byref(c2), float(angle_tol), _ptr(out), x1 - x0,
+              dev, _stream_ptr() if dev else None))
     return out
 
 

@@ -226,16 +226,15 @@ template <class T> int dispmap_transform_launch(int mode, const double* m9, int 
 int warp_launch(const vwb200_warp_params& p, const float* in, int w, int h, ptrdiff_t ip, const DispF* disp, int dw, int dh, ptrdiff_t dp,
                 int x0, int y0, float* out, int ow, int oh, ptrdiff_t op, cudaStream_t st);
 struct TriCam;
-// camera_transform (Camera/CameraTransform.h:43-183): reverse(p) = src.point_to_pixel(dst.pixel_to_vector(p) + C).  masked: the
-// pixels are PixelMask<float> {value, valid} float pairs (pitches in pairs; bilinear only, edge_value[2] for VWB200_EDGE_VALUE).
-// fail (device, 0 and ULLONG_MAX on entry): [0] is set and [1] lowered to the row-major window index of every pixel whose
-// point_to_pixel check fails.
-int camera_warp_launch(int masked, int interp, int edge, const float* edge_value, const TriCam& src, const TriCam& dst, const float* in, int w,
-                       int h, ptrdiff_t ip, int x0, int y0, float* out, int ow, int oh, ptrdiff_t op, unsigned long long* fail, cudaStream_t st);
-// camera_transform as above from a CAHV or CAHVOR src into a CAHV dst (no point_to_pixel check: the CAHV family has none)
 struct CahvCam;
-int cahv_warp_launch(int masked, int interp, int edge, const float* edge_value, const CahvCam& src, const CahvCam& dst, const float* in, int w,
-                     int h, ptrdiff_t ip, int x0, int y0, float* out, int ow, int oh, ptrdiff_t op, cudaStream_t st);
+// camera_transform (Camera/CameraTransform.h:43-183): reverse(p) = src.point_to_pixel(dst.pixel_to_vector(p) + C) between two
+// pinhole cameras (Cam = TriCam), or from a CAHV or CAHVOR src into a CAHV dst (Cam = CahvCam).  masked: the pixels are
+// PixelMask<float> {value, valid} float pairs (pitches in pairs; bilinear only, edge_value[2] for VWB200_EDGE_VALUE).
+// fail (device, 0 and ULLONG_MAX on entry): [0] is set and [1] lowered to the row-major window index of every pixel whose
+// point_to_pixel check fails (pinhole cameras only: the CAHV family has no check).
+template <class Cam>
+int camera_warp_launch(int masked, int interp, int edge, const float* edge_value, const Cam& src, const Cam& dst, const float* in, int w, int h,
+                       ptrdiff_t ip, int x0, int y0, float* out, int ow, int oh, ptrdiff_t op, unsigned long long* fail, cudaStream_t st);
 // compute_transformed_bbox_fast (Image/Transform.h:271-315) of the ROI (x0, y0, x1, y1) through CameraTransform(src, dst)::forward
 // into keys4 (device, fkey of min x, min y, max x, max y; the caller seeds them with BBox2f's initial bounds); fail as above,
 // with the perimeter index in the reference's loop order
@@ -252,23 +251,20 @@ template <class T> int fill_holes_grass_launch(const T* in, int w, int h, ptrdif
 // (row-major), the center, the pixel pitch, the intrinsics the lens normalises by, and the Tsai parameters when tsai != 0;
 // P is the 3 x 4 camera matrix K * [uvw * transpose(R) | uvw * (-transpose(R)) * C] (row-major) that point_to_pixel applies
 struct TriCam { double inv[9], c[3], pitch, fu, fv, cu, cv, k[5]; int tsai; double P[12]; };
-// stats: 5 x 8 bytes of zeroed device scratch -- [0] error sum (double), [1] max error (double bits), [2] points,
-// [3] divergent, [4] Tsai Newton-Raphson iterations; form (a) fills [4] only.  xyz pitches count {x, y, z} pixels.
-template <class T> int stereo_triangulate_launch(const T* in, ptrdiff_t ip, int x0, int y0, int ow, int oh, const TriCam& c0, const TriCam& c1,
-                                                 double tol, double* xyz, ptrdiff_t xp, unsigned long long* stats, cudaStream_t st);
-int stereo_model_launch(const DispF* in, int w, int h, ptrdiff_t ip, const TriCam& c0, const TriCam& c1, double tol, double* xyz, ptrdiff_t xp,
-                        double* err, ptrdiff_t ep, unsigned long long* stats, cudaStream_t st);
 // what CAHVModel / CAHVORModel::pixel_to_vector, point_to_pixel and camera_center need (Camera/CAHVModel.cc:167-189,
 // CAHVORModel.cc:297-350, 431-448): the six vectors (O and R unused unless cahvor), cahvor != 0 for the CAHVOR model, and
 // flip != 0 where dot_prod(cross_prod(V, H), A) < 0 (the host evaluates it once per call in the reference's order)
 struct CahvCam { double C[3], A[3], H[3], V[3], O[3], R[3]; int cahvor, flip; };
-// stereo_triangulate / StereoModel as above through CAHV or CAHVOR cameras (each independently): stats is 6 x 8 bytes of
-// zeroed device scratch, [0]-[3] as above, [5] the CAHVOR Newton iterations of both rays of every triangulated pixel
-template <class T> int cahv_stereo_triangulate_launch(const T* in, ptrdiff_t ip, int x0, int y0, int ow, int oh, const CahvCam& c0,
-                                                      const CahvCam& c1, double tol, double* xyz, ptrdiff_t xp, unsigned long long* stats,
-                                                      cudaStream_t st);
-int cahv_stereo_model_launch(const DispF* in, int w, int h, ptrdiff_t ip, const CahvCam& c0, const CahvCam& c1, double tol, double* xyz,
-                             ptrdiff_t xp, double* err, ptrdiff_t ep, unsigned long long* stats, cudaStream_t st);
+// Cam = TriCam (two pinhole cameras) or CahvCam (two CAHV or CAHVOR cameras, each independently).  stats: 5 x 8 bytes of
+// zeroed device scratch -- [0] error sum (double), [1] max error (double bits), [2] points, [3] divergent, [4] the Newton
+// iterations of both rays of every triangulated pixel (Tsai Newton-Raphson or CAHVOR Newton passes); form (a) fills [4] only.
+// xyz pitches count {x, y, z} pixels.
+template <class Cam, class T>
+int stereo_triangulate_launch(const T* in, ptrdiff_t ip, int x0, int y0, int ow, int oh, const Cam& c0, const Cam& c1, double tol, double* xyz,
+                              ptrdiff_t xp, unsigned long long* stats, cudaStream_t st);
+template <class Cam>
+int stereo_model_launch(const DispF* in, int w, int h, ptrdiff_t ip, const Cam& c0, const Cam& c1, double tol, double* xyz, ptrdiff_t xp,
+                        double* err, ptrdiff_t ep, unsigned long long* stats, cudaStream_t st);
 // in may be out (same pitch); *rejected (device) is added to
 int universe_radius_launch(const double* in, int w, int h, ptrdiff_t ip, const double* origin, double near_r, double far_r, double* out,
                            ptrdiff_t op, unsigned long long* rejected, cudaStream_t st);

@@ -1897,19 +1897,10 @@ static int pinhole_build(const char* what, const vwb200_pinhole& p, TriCam* c) {
   return VWB200_OK;
 }
 
-// both cameras, then the device; tol is are_nearly_parallel's (StereoModel.cc:81-83)
-static int cameras_open(const char* what, const vwb200_pinhole* cam1, const vwb200_pinhole* cam2, double angle_tol, TriCam* c0, TriCam* c1,
-                        double* tol) {
-  VWB_TRY(pinhole_build(what, *cam1, c0));
-  VWB_TRY(pinhole_build(what, *cam2, c1));
-  *tol = angle_tol > 0 ? angle_tol : 1e-4;
-  return ensure_device();
-}
-
-// n (5, or 6 with the CAHVOR counter) zeroed device statistics of one call
-static int tri_stats_open(AbiCall& c, unsigned long long** d, int n = 5) {
-  VWB_TRY(c.ar.alloc(d, n));
-  VWB_CUDA(cudaMemsetAsync(*d, 0, n * sizeof(unsigned long long), c.st));
+// the five zeroed device statistics of one call
+static int tri_stats_open(AbiCall& c, unsigned long long** d) {
+  VWB_TRY(c.ar.alloc(d, 5));
+  VWB_CUDA(cudaMemsetAsync(*d, 0, 5 * sizeof(unsigned long long), c.st));
   return VWB200_OK;
 }
 
@@ -1938,75 +1929,6 @@ static int model_points_args(const char* what, const float* disparity, int w, in
     set_error("%s: the disparity, xyz and error rasters overlap", what);
     return VWB200_EARG;
   }
-  return VWB200_OK;
-}
-
-int vwb200_stereo_triangulate(int pixel_type, const void* disparity, int w, int h, ptrdiff_t pitch, int x0, int y0, int ow, int oh,
-                              const vwb200_pinhole* cam1, const vwb200_pinhole* cam2, double angle_tol, double* xyz, ptrdiff_t xyz_pitch,
-                              int on_device, void* stream) {
-  t_tri_stats = vwb200_triangulation_stats{0, 0, 0.0, 0.0, 0};
-  const char* what = "stereo_triangulate";
-  if (!disparity || !xyz) { set_error("%s: null disparity or output", what); return VWB200_EARG; }
-  if (pixel_type != VWB200_DISP_I32 && pixel_type != VWB200_DISP_F32) { set_error("%s: unknown pixel type %d", what, pixel_type); return VWB200_EARG; }
-  VWB_TRY(pinhole_check(what, cam1));
-  VWB_TRY(pinhole_check(what, cam2));
-  VWB_TRY(triangulate_args(what, disparity, w, h, pitch, x0, y0, ow, oh, xyz, xyz_pitch));
-  TriCam c0, c1;
-  double tol;
-  VWB_TRY(cameras_open(what, cam1, cam2, angle_tol, &c0, &c1, &tol));
-  AbiCall c;
-  VWB_TRY(c.open(stream, on_device));
-  Pt3* dxyz; ptrdiff_t dxp;
-  VWB_TRY(c.out((Pt3*)xyz, ow, oh, xyz_pitch, on_device, &dxyz, &dxp));
-  unsigned long long* dst;
-  VWB_TRY(tri_stats_open(c, &dst));
-  // only the window is read: stage that alone
-  if (pixel_type == VWB200_DISP_I32) {
-    const vwb200_dispi* din; ptrdiff_t dp;
-    VWB_TRY(c.in((const vwb200_dispi*)disparity + (ptrdiff_t)y0 * pitch + x0, ow, oh, pitch, on_device, &din, &dp));
-    VWB_TRY(stereo_triangulate_launch(din, dp, x0, y0, ow, oh, c0, c1, tol, (double*)dxyz, dxp, dst, c.st));
-  } else {
-    const DispF* din; ptrdiff_t dp;
-    VWB_TRY(c.in((const DispF*)disparity + (ptrdiff_t)y0 * pitch + x0, ow, oh, pitch, on_device, &din, &dp));
-    VWB_TRY(stereo_triangulate_launch(din, dp, x0, y0, ow, oh, c0, c1, tol, (double*)dxyz, dxp, dst, c.st));
-  }
-  unsigned long long s[5];
-  VWB_CUDA(cudaMemcpyAsync(s, dst, sizeof s, cudaMemcpyDeviceToHost, c.st));
-  VWB_TRY(c.finish());
-  t_tri_stats.tsai_iterations = (long long)s[4];
-  return VWB200_OK;
-}
-
-int vwb200_stereo_model_points(const float* disparity, int w, int h, ptrdiff_t pitch, const vwb200_pinhole* cam1,
-                               const vwb200_pinhole* cam2, double angle_tol, double* xyz, ptrdiff_t xyz_pitch, double* error,
-                               ptrdiff_t error_pitch, int on_device, void* stream) {
-  t_tri_stats = vwb200_triangulation_stats{0, 0, 0.0, 0.0, 0};
-  const char* what = "StereoModel";
-  if (!disparity || !xyz || !error) { set_error("%s: null disparity or output", what); return VWB200_EARG; }
-  VWB_TRY(pinhole_check(what, cam1));
-  VWB_TRY(pinhole_check(what, cam2));
-  VWB_TRY(model_points_args(what, disparity, w, h, pitch, xyz, xyz_pitch, error, error_pitch));
-  TriCam c0, c1;
-  double tol;
-  VWB_TRY(cameras_open(what, cam1, cam2, angle_tol, &c0, &c1, &tol));
-  AbiCall c;
-  VWB_TRY(c.open(stream, on_device));
-  const DispF* din; ptrdiff_t dp;
-  VWB_TRY(c.in((const DispF*)disparity, w, h, pitch, on_device, &din, &dp));
-  Pt3* dxyz; ptrdiff_t dxp;
-  VWB_TRY(c.out((Pt3*)xyz, w, h, xyz_pitch, on_device, &dxyz, &dxp));
-  double* derr; ptrdiff_t dep;
-  VWB_TRY(c.out(error, w, h, error_pitch, on_device, &derr, &dep));
-  unsigned long long* dst;
-  VWB_TRY(tri_stats_open(c, &dst));
-  VWB_TRY(stereo_model_launch(din, w, h, dp, c0, c1, tol, (double*)dxyz, dxp, derr, dep, dst, c.st));
-  unsigned long long s[5];
-  VWB_CUDA(cudaMemcpyAsync(s, dst, sizeof s, cudaMemcpyDeviceToHost, c.st));
-  VWB_TRY(c.finish());
-  double sum, mx;
-  std::memcpy(&sum, &s[0], sizeof sum);
-  std::memcpy(&mx, &s[1], sizeof mx);
-  t_tri_stats = vwb200_triangulation_stats{(long long)s[2], (long long)s[3], mx, sum, (long long)s[4]};
   return VWB200_OK;
 }
 
@@ -2115,8 +2037,8 @@ int vwb200_pinhole_epipolar(const vwb200_pinhole* cam0, const vwb200_pinhole* ca
 struct MaskF { float v, valid; };                                // PixelMask<float>
 
 // CameraTransform's VW_ASSERT (CameraTransform.h:53, 66): both cameras at one center
-static int same_center(const char* what, const TriCam& a, const TriCam& b) {
-  if (a.c[0] == b.c[0] && a.c[1] == b.c[1] && a.c[2] == b.c[2]) return VWB200_OK;
+static int same_center(const char* what, const double* a, const double* b) {
+  if (a[0] == b[0] && a[1] == b[1] && a[2] == b[2]) return VWB200_OK;
   set_error("%s: CameraTransformFunctor: Camera transformation require that the camera center is always the same for both cameras.", what);
   return VWB200_ELOGIC;
 }
@@ -2197,8 +2119,8 @@ int vwb200_resize_epipolar_cameras_to_fit(const vwb200_pinhole* cam1, const vwb2
   VWB_TRY(pinhole_build(what, *cam2, &cam[1]));
   VWB_TRY(pinhole_build(what, *epi1, &epi[0]));
   VWB_TRY(pinhole_build(what, *epi2, &epi[1]));
-  VWB_TRY(same_center(what, cam[0], epi[0]));
-  VWB_TRY(same_center(what, cam[1], epi[1]));
+  VWB_TRY(same_center(what, cam[0].c, epi[0].c));
+  VWB_TRY(same_center(what, cam[1].c, epi[1].c));
   VWB_TRY(ensure_device());
   AbiCall c;
   VWB_TRY(c.open(stream, 0));
@@ -2264,38 +2186,6 @@ static int camera_transform_stage(AbiCall& c, bool masked, const void* in, int w
   return c.out((float*)out, ow, oh, opitch, on_device, dout, dop);
 }
 
-int vwb200_camera_transform(const vwb200_pinhole* src, const vwb200_pinhole* dst, int pixel_type, int interp, int edge, const float edge_value[2],
-                            const void* in, int w, int h, ptrdiff_t pitch, int x0, int y0, void* out, int ow, int oh, ptrdiff_t opitch,
-                            int on_device, void* stream) {
-  const char* what = "camera_transform";
-  if (!in || !out) { set_error("%s: null input or output", what); return VWB200_EARG; }
-  VWB_TRY(pinhole_check(what, src));
-  VWB_TRY(pinhole_check(what, dst));
-  VWB_TRY(camera_transform_args(what, pixel_type, interp, edge, edge_value, in, w, h, pitch, x0, y0, out, ow, oh, opitch));
-  const bool masked = pixel_type == VWB200_PIXEL_MASK_F32;
-  const float ev[2] = {edge_value ? edge_value[0] : 0.0f, edge_value ? edge_value[1] : 0.0f};
-  TriCam s, d;
-  VWB_TRY(pinhole_build(what, *src, &s));
-  VWB_TRY(pinhole_build(what, *dst, &d));
-  VWB_TRY(same_center(what, s, d));
-  VWB_TRY(ensure_device());
-  AbiCall c;
-  VWB_TRY(c.open(stream, on_device));
-  const float* din; ptrdiff_t dp;
-  float* dout; ptrdiff_t dop;
-  VWB_TRY(camera_transform_stage(c, masked, in, w, h, pitch, out, ow, oh, opitch, on_device, &din, &dp, &dout, &dop));
-  unsigned long long* fail;
-  VWB_TRY(c.ar.alloc(&fail, 2));
-  const unsigned long long finit[2] = {0, ULLONG_MAX};
-  VWB_CUDA(cudaMemcpyAsync(fail, finit, sizeof finit, cudaMemcpyHostToDevice, c.st));
-  VWB_TRY(camera_warp_launch(masked, interp, edge, ev, s, d, din, w, h, dp, x0, y0, dout, ow, oh, dop, fail, c.st));
-  unsigned long long f[2];
-  VWB_CUDA(cudaMemcpyAsync(f, fail, sizeof f, cudaMemcpyDeviceToHost, c.st));
-  VWB_TRY(c.finish());
-  if (f[0]) return projection_error(what, x0 + (long long)(f[1] % (unsigned long long)ow), y0 + (long long)(f[1] / (unsigned long long)ow));
-  return VWB200_OK;
-}
-
 // ---- the view -------------------------------------------------------------------------------------
 // ---- CAHV / CAHVOR cameras (Camera/CAHVModel.cc, CAHVORModel.cc, CameraTransform.h, StereoModel.cc:121-122) ---------------------
 // The host restatement of the camera math (linearize_camera calls pixel_to_vector); cahv.cuh is the device one.  x86-64 host
@@ -2316,15 +2206,6 @@ static int cahv_check(const char* what, const vwb200_cahv* c) {
   if (!c) { set_error("%s: null camera", what); return VWB200_EARG; }
   if (c->model != VWB200_CAMERA_CAHV && c->model != VWB200_CAMERA_CAHVOR) { set_error("%s: unknown camera model %d", what, c->model); return VWB200_EARG; }
   return VWB200_OK;
-}
-
-static CahvCam cahv_build(const vwb200_cahv& c) {
-  CahvCam d;
-  std::memcpy(d.C, c.C, sizeof d.C); std::memcpy(d.A, c.A, sizeof d.A); std::memcpy(d.H, c.H, sizeof d.H);
-  std::memcpy(d.V, c.V, sizeof d.V); std::memcpy(d.O, c.O, sizeof d.O); std::memcpy(d.R, c.R, sizeof d.R);
-  d.cahvor = c.model == VWB200_CAMERA_CAHVOR;
-  d.flip = cahv_left_handed(c);
-  return d;
 }
 
 // CAHVORModel::pixel_to_vector(pix), the overload without partial derivatives (CAHVORModel.cc:297-348)
@@ -2493,77 +2374,93 @@ int vwb200_pinhole_to_cahv(const vwb200_pinhole* pin, vwb200_cahv* out) {
   return VWB200_OK;
 }
 
-int vwb200_cahv_camera_transform(const vwb200_cahv* src, const vwb200_cahv* dst, int pixel_type, int interp, int edge, const float edge_value[2],
-                                 const void* in, int w, int h, ptrdiff_t pitch, int x0, int y0, void* out, int ow, int oh, ptrdiff_t opitch,
-                                 int on_device, void* stream) {
-  const char* what = "camera_transform";
-  if (!in || !out) { set_error("%s: null input or output", what); return VWB200_EARG; }
-  VWB_TRY(cahv_check(what, src));
-  VWB_TRY(cahv_check(what, dst));
-  VWB_TRY(camera_transform_args(what, pixel_type, interp, edge, edge_value, in, w, h, pitch, x0, y0, out, ow, oh, opitch));
-  if (dst->model != VWB200_CAMERA_CAHV) { set_error("%s: the destination camera must be CAHV (a CAHVOR one has no device form)", what); return VWB200_ENOIMPL; }
-  if (!(src->C[0] == dst->C[0] && src->C[1] == dst->C[1] && src->C[2] == dst->C[2])) {
-    set_error("%s: CameraTransformFunctor: Camera transformation require that the camera center is always the same for both cameras.", what);
-    return VWB200_ELOGIC;
+// ---- stereo_triangulate, StereoModel and camera_transform through either camera family -----------------------------------
+// What these calls need to know of a family: its C ABI and device cameras, the argument check, build (VWB200_ELOGIC / EMATH for
+// a pinhole camera the reference cannot construct), the center, the statistic that receives the Newton iterations, and which
+// camera_transform destinations have a device form.  The family bodies are templates, so they sit in an extern "C++" block.
+extern "C++" {
+struct PinholeFamily {
+  using Abi = vwb200_pinhole;
+  using Dev = TriCam;
+  static constexpr auto check = pinhole_check;
+  static constexpr auto build = pinhole_build;
+  static const double* center(const TriCam& c) { return c.c; }
+  static constexpr long long vwb200_triangulation_stats::*iterations = &vwb200_triangulation_stats::tsai_iterations;
+  static int transform_dst(const char*, const vwb200_pinhole&) { return VWB200_OK; }
+};
+struct CahvFamily {
+  using Abi = vwb200_cahv;
+  using Dev = CahvCam;
+  static constexpr auto check = cahv_check;
+  static int build(const char*, const vwb200_cahv& c, CahvCam* d) {
+    std::memcpy(d->C, c.C, sizeof d->C); std::memcpy(d->A, c.A, sizeof d->A); std::memcpy(d->H, c.H, sizeof d->H);
+    std::memcpy(d->V, c.V, sizeof d->V); std::memcpy(d->O, c.O, sizeof d->O); std::memcpy(d->R, c.R, sizeof d->R);
+    d->cahvor = c.model == VWB200_CAMERA_CAHVOR;
+    d->flip = cahv_left_handed(c);
+    return VWB200_OK;
   }
-  const bool masked = pixel_type == VWB200_PIXEL_MASK_F32;
-  const float ev[2] = {edge_value ? edge_value[0] : 0.0f, edge_value ? edge_value[1] : 0.0f};
-  const CahvCam s = cahv_build(*src), d = cahv_build(*dst);
-  VWB_TRY(ensure_device());
-  AbiCall c;
-  VWB_TRY(c.open(stream, on_device));
-  const float* din; ptrdiff_t dp;
-  float* dout; ptrdiff_t dop;
-  VWB_TRY(camera_transform_stage(c, masked, in, w, h, pitch, out, ow, oh, opitch, on_device, &din, &dp, &dout, &dop));
-  VWB_TRY(cahv_warp_launch(masked, interp, edge, ev, s, d, din, w, h, dp, x0, y0, dout, ow, oh, dop, c.st));
-  return c.finish();
-}
+  static const double* center(const CahvCam& c) { return c.C; }
+  static constexpr long long vwb200_triangulation_stats::*iterations = &vwb200_triangulation_stats::cahvor_iterations;
+  // K8 compiles the destination's ray without the CAHVOR Newton loop
+  static int transform_dst(const char* what, const vwb200_cahv& c) {
+    if (c.model == VWB200_CAMERA_CAHV) return VWB200_OK;
+    set_error("%s: the destination camera must be CAHV (a CAHVOR one has no device form)", what);
+    return VWB200_ENOIMPL;
+  }
+};
 
-int vwb200_cahv_stereo_triangulate(int pixel_type, const void* disparity, int w, int h, ptrdiff_t pitch, int x0, int y0, int ow, int oh,
-                                   const vwb200_cahv* cam1, const vwb200_cahv* cam2, double angle_tol, double* xyz, ptrdiff_t xyz_pitch,
-                                   int on_device, void* stream) {
-  t_tri_stats = vwb200_triangulation_stats{0, 0, 0.0, 0.0, 0, 0};
+template <class F>
+static int stereo_triangulate_family(int pixel_type, const void* disparity, int w, int h, ptrdiff_t pitch, int x0, int y0, int ow, int oh,
+                                     const typename F::Abi* cam1, const typename F::Abi* cam2, double angle_tol, double* xyz,
+                                     ptrdiff_t xyz_pitch, int on_device, void* stream) {
+  t_tri_stats = vwb200_triangulation_stats{};
   const char* what = "stereo_triangulate";
   if (!disparity || !xyz) { set_error("%s: null disparity or output", what); return VWB200_EARG; }
   if (pixel_type != VWB200_DISP_I32 && pixel_type != VWB200_DISP_F32) { set_error("%s: unknown pixel type %d", what, pixel_type); return VWB200_EARG; }
-  VWB_TRY(cahv_check(what, cam1));
-  VWB_TRY(cahv_check(what, cam2));
+  VWB_TRY(F::check(what, cam1));
+  VWB_TRY(F::check(what, cam2));
   VWB_TRY(triangulate_args(what, disparity, w, h, pitch, x0, y0, ow, oh, xyz, xyz_pitch));
-  const CahvCam c0 = cahv_build(*cam1), c1 = cahv_build(*cam2);
-  const double tol = angle_tol > 0 ? angle_tol : 1e-4;
+  typename F::Dev c0, c1;
+  VWB_TRY(F::build(what, *cam1, &c0));
+  VWB_TRY(F::build(what, *cam2, &c1));
+  const double tol = angle_tol > 0 ? angle_tol : 1e-4;            // are_nearly_parallel's (StereoModel.cc:81-83)
   VWB_TRY(ensure_device());
   AbiCall c;
   VWB_TRY(c.open(stream, on_device));
   Pt3* dxyz; ptrdiff_t dxp;
   VWB_TRY(c.out((Pt3*)xyz, ow, oh, xyz_pitch, on_device, &dxyz, &dxp));
   unsigned long long* dst;
-  VWB_TRY(tri_stats_open(c, &dst, 6));
+  VWB_TRY(tri_stats_open(c, &dst));
+  // only the window is read: stage that alone
   if (pixel_type == VWB200_DISP_I32) {
     const vwb200_dispi* din; ptrdiff_t dp;
     VWB_TRY(c.in((const vwb200_dispi*)disparity + (ptrdiff_t)y0 * pitch + x0, ow, oh, pitch, on_device, &din, &dp));
-    VWB_TRY(cahv_stereo_triangulate_launch(din, dp, x0, y0, ow, oh, c0, c1, tol, (double*)dxyz, dxp, dst, c.st));
+    VWB_TRY(stereo_triangulate_launch(din, dp, x0, y0, ow, oh, c0, c1, tol, (double*)dxyz, dxp, dst, c.st));
   } else {
     const DispF* din; ptrdiff_t dp;
     VWB_TRY(c.in((const DispF*)disparity + (ptrdiff_t)y0 * pitch + x0, ow, oh, pitch, on_device, &din, &dp));
-    VWB_TRY(cahv_stereo_triangulate_launch(din, dp, x0, y0, ow, oh, c0, c1, tol, (double*)dxyz, dxp, dst, c.st));
+    VWB_TRY(stereo_triangulate_launch(din, dp, x0, y0, ow, oh, c0, c1, tol, (double*)dxyz, dxp, dst, c.st));
   }
-  unsigned long long s[6];
+  unsigned long long s[5];
   VWB_CUDA(cudaMemcpyAsync(s, dst, sizeof s, cudaMemcpyDeviceToHost, c.st));
   VWB_TRY(c.finish());
-  t_tri_stats.cahvor_iterations = (long long)s[5];
+  t_tri_stats.*F::iterations = (long long)s[4];
   return VWB200_OK;
 }
 
-int vwb200_cahv_stereo_model_points(const float* disparity, int w, int h, ptrdiff_t pitch, const vwb200_cahv* cam1, const vwb200_cahv* cam2,
-                                    double angle_tol, double* xyz, ptrdiff_t xyz_pitch, double* error, ptrdiff_t error_pitch, int on_device,
-                                    void* stream) {
-  t_tri_stats = vwb200_triangulation_stats{0, 0, 0.0, 0.0, 0, 0};
+template <class F>
+static int stereo_model_points_family(const float* disparity, int w, int h, ptrdiff_t pitch, const typename F::Abi* cam1,
+                                      const typename F::Abi* cam2, double angle_tol, double* xyz, ptrdiff_t xyz_pitch, double* error,
+                                      ptrdiff_t error_pitch, int on_device, void* stream) {
+  t_tri_stats = vwb200_triangulation_stats{};
   const char* what = "StereoModel";
   if (!disparity || !xyz || !error) { set_error("%s: null disparity or output", what); return VWB200_EARG; }
-  VWB_TRY(cahv_check(what, cam1));
-  VWB_TRY(cahv_check(what, cam2));
+  VWB_TRY(F::check(what, cam1));
+  VWB_TRY(F::check(what, cam2));
   VWB_TRY(model_points_args(what, disparity, w, h, pitch, xyz, xyz_pitch, error, error_pitch));
-  const CahvCam c0 = cahv_build(*cam1), c1 = cahv_build(*cam2);
+  typename F::Dev c0, c1;
+  VWB_TRY(F::build(what, *cam1, &c0));
+  VWB_TRY(F::build(what, *cam2, &c1));
   const double tol = angle_tol > 0 ? angle_tol : 1e-4;
   VWB_TRY(ensure_device());
   AbiCall c;
@@ -2575,16 +2472,94 @@ int vwb200_cahv_stereo_model_points(const float* disparity, int w, int h, ptrdif
   double* derr; ptrdiff_t dep;
   VWB_TRY(c.out(error, w, h, error_pitch, on_device, &derr, &dep));
   unsigned long long* dst;
-  VWB_TRY(tri_stats_open(c, &dst, 6));
-  VWB_TRY(cahv_stereo_model_launch(din, w, h, dp, c0, c1, tol, (double*)dxyz, dxp, derr, dep, dst, c.st));
-  unsigned long long s[6];
+  VWB_TRY(tri_stats_open(c, &dst));
+  VWB_TRY(stereo_model_launch(din, w, h, dp, c0, c1, tol, (double*)dxyz, dxp, derr, dep, dst, c.st));
+  unsigned long long s[5];
   VWB_CUDA(cudaMemcpyAsync(s, dst, sizeof s, cudaMemcpyDeviceToHost, c.st));
   VWB_TRY(c.finish());
   double sum, mx;
   std::memcpy(&sum, &s[0], sizeof sum);
   std::memcpy(&mx, &s[1], sizeof mx);
-  t_tri_stats = vwb200_triangulation_stats{(long long)s[2], (long long)s[3], mx, sum, 0, (long long)s[5]};
+  t_tri_stats = vwb200_triangulation_stats{(long long)s[2], (long long)s[3], mx, sum, 0, 0};
+  t_tri_stats.*F::iterations = (long long)s[4];
   return VWB200_OK;
+}
+
+template <class F>
+static int camera_transform_family(const typename F::Abi* src, const typename F::Abi* dst, int pixel_type, int interp, int edge,
+                                   const float* edge_value, const void* in, int w, int h, ptrdiff_t pitch, int x0, int y0, void* out, int ow,
+                                   int oh, ptrdiff_t opitch, int on_device, void* stream) {
+  const char* what = "camera_transform";
+  if (!in || !out) { set_error("%s: null input or output", what); return VWB200_EARG; }
+  VWB_TRY(F::check(what, src));
+  VWB_TRY(F::check(what, dst));
+  VWB_TRY(camera_transform_args(what, pixel_type, interp, edge, edge_value, in, w, h, pitch, x0, y0, out, ow, oh, opitch));
+  VWB_TRY(F::transform_dst(what, *dst));
+  const bool masked = pixel_type == VWB200_PIXEL_MASK_F32;
+  const float ev[2] = {edge_value ? edge_value[0] : 0.0f, edge_value ? edge_value[1] : 0.0f};
+  typename F::Dev s, d;
+  VWB_TRY(F::build(what, *src, &s));
+  VWB_TRY(F::build(what, *dst, &d));
+  VWB_TRY(same_center(what, F::center(s), F::center(d)));
+  VWB_TRY(ensure_device());
+  AbiCall c;
+  VWB_TRY(c.open(stream, on_device));
+  const float* din; ptrdiff_t dp;
+  float* dout; ptrdiff_t dop;
+  VWB_TRY(camera_transform_stage(c, masked, in, w, h, pitch, out, ow, oh, opitch, on_device, &din, &dp, &dout, &dop));
+  unsigned long long* fail;
+  VWB_TRY(c.ar.alloc(&fail, 2));
+  const unsigned long long finit[2] = {0, ULLONG_MAX};
+  VWB_CUDA(cudaMemcpyAsync(fail, finit, sizeof finit, cudaMemcpyHostToDevice, c.st));
+  VWB_TRY(camera_warp_launch(masked, interp, edge, ev, s, d, din, w, h, dp, x0, y0, dout, ow, oh, dop, fail, c.st));
+  unsigned long long f[2];
+  VWB_CUDA(cudaMemcpyAsync(f, fail, sizeof f, cudaMemcpyDeviceToHost, c.st));
+  VWB_TRY(c.finish());
+  if (f[0]) return projection_error(what, x0 + (long long)(f[1] % (unsigned long long)ow), y0 + (long long)(f[1] / (unsigned long long)ow));
+  return VWB200_OK;
+}
+}  // extern "C++"
+
+int vwb200_stereo_triangulate(int pixel_type, const void* disparity, int w, int h, ptrdiff_t pitch, int x0, int y0, int ow, int oh,
+                              const vwb200_pinhole* cam1, const vwb200_pinhole* cam2, double angle_tol, double* xyz, ptrdiff_t xyz_pitch,
+                              int on_device, void* stream) {
+  return stereo_triangulate_family<PinholeFamily>(pixel_type, disparity, w, h, pitch, x0, y0, ow, oh, cam1, cam2, angle_tol, xyz, xyz_pitch,
+                                                  on_device, stream);
+}
+
+int vwb200_cahv_stereo_triangulate(int pixel_type, const void* disparity, int w, int h, ptrdiff_t pitch, int x0, int y0, int ow, int oh,
+                                   const vwb200_cahv* cam1, const vwb200_cahv* cam2, double angle_tol, double* xyz, ptrdiff_t xyz_pitch,
+                                   int on_device, void* stream) {
+  return stereo_triangulate_family<CahvFamily>(pixel_type, disparity, w, h, pitch, x0, y0, ow, oh, cam1, cam2, angle_tol, xyz, xyz_pitch,
+                                               on_device, stream);
+}
+
+int vwb200_stereo_model_points(const float* disparity, int w, int h, ptrdiff_t pitch, const vwb200_pinhole* cam1,
+                               const vwb200_pinhole* cam2, double angle_tol, double* xyz, ptrdiff_t xyz_pitch, double* error,
+                               ptrdiff_t error_pitch, int on_device, void* stream) {
+  return stereo_model_points_family<PinholeFamily>(disparity, w, h, pitch, cam1, cam2, angle_tol, xyz, xyz_pitch, error, error_pitch,
+                                                   on_device, stream);
+}
+
+int vwb200_cahv_stereo_model_points(const float* disparity, int w, int h, ptrdiff_t pitch, const vwb200_cahv* cam1, const vwb200_cahv* cam2,
+                                    double angle_tol, double* xyz, ptrdiff_t xyz_pitch, double* error, ptrdiff_t error_pitch, int on_device,
+                                    void* stream) {
+  return stereo_model_points_family<CahvFamily>(disparity, w, h, pitch, cam1, cam2, angle_tol, xyz, xyz_pitch, error, error_pitch, on_device,
+                                                stream);
+}
+
+int vwb200_camera_transform(const vwb200_pinhole* src, const vwb200_pinhole* dst, int pixel_type, int interp, int edge, const float edge_value[2],
+                            const void* in, int w, int h, ptrdiff_t pitch, int x0, int y0, void* out, int ow, int oh, ptrdiff_t opitch,
+                            int on_device, void* stream) {
+  return camera_transform_family<PinholeFamily>(src, dst, pixel_type, interp, edge, edge_value, in, w, h, pitch, x0, y0, out, ow, oh, opitch,
+                                                on_device, stream);
+}
+
+int vwb200_cahv_camera_transform(const vwb200_cahv* src, const vwb200_cahv* dst, int pixel_type, int interp, int edge, const float edge_value[2],
+                                 const void* in, int w, int h, ptrdiff_t pitch, int x0, int y0, void* out, int ow, int oh, ptrdiff_t opitch,
+                                 int on_device, void* stream) {
+  return camera_transform_family<CahvFamily>(src, dst, pixel_type, interp, edge, edge_value, in, w, h, pitch, x0, y0, out, ow, oh, opitch,
+                                             on_device, stream);
 }
 
 int vwb200_corr_create(const vwb200_corr_params* p, vwb200_corr** out) {

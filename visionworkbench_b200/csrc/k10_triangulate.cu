@@ -1,11 +1,11 @@
-// k10_triangulate.cu -- K10: dense two-camera triangulation of a disparity through pinhole cameras (Stereo/StereoView.h:74-130,
-// Stereo/StereoModel.cc:35-147, 254-309, Camera/PinholeModel.cc:422-434, Camera/LensDistortion.cc:258-400,
-// Math/NewtonRaphson.cc:58-119), and UniverseRadiusFunc on a Vector3 image (StereoView.h:139-186).
+// k10_triangulate.cu -- K10: dense two-camera triangulation of a disparity through pinhole or CAHV / CAHVOR cameras
+// (Stereo/StereoView.h:74-130, Stereo/StereoModel.cc:35-147, 254-309, Camera/PinholeModel.cc:422-434,
+// Camera/LensDistortion.cc:258-400, Math/NewtonRaphson.cc:58-119), and UniverseRadiusFunc on a Vector3 image (StereoView.h:139-186).
 //
 // One thread per pixel, grid-stride over rows.  Each warp stages its 32 {x, y, z} results in shared memory and stores them as
-// three contiguous 256-byte runs.  The cameras are kernel parameters (TriCam: the inverse camera transform the host builds
-// once per call, the center, the pixel pitch and the lens); the camera math is pinhole.cuh's, bit for bit the reference's.
-// k10_triangulate_cahv_kernel<T, MODEL> is the same pass through CAHV / CAHVOR cameras (cahv.cuh): only the rays differ.
+// three contiguous 256-byte runs.  The cameras are kernel parameters: a TriCam (the inverse camera transform the host builds
+// once per call, the center, the pixel pitch and the lens) with pinhole.cuh's camera math, or a CahvCam with cahv.cuh's, both
+// bit for bit the reference's.
 #include "cahv.cuh"
 
 namespace vwb200 {
@@ -30,27 +30,26 @@ __device__ __forceinline__ V3 intersect(const V3 C0, const V3 C1, const V3 d0, c
   return r;
 }
 
-// StereoModel::operator()(pix1, pix2, errorVec) for two pinhole cameras
-template <bool TSAI>
-__device__ __forceinline__ V3 triangulate(const TriCam& c0, const TriCam& c1, double tol, double l0, double l1, double r0, double r1,
-                                          V3* err, int* iters) {
+// each family's camera_center and pixel_to_vector: a pinhole camera's through pinhole.cuh (ITER: the Tsai Newton-Raphson may run),
+// a CAHV / CAHVOR camera's through cahv.cuh (ITER: the CAHVOR Newton loop may run); *iters counts the iterations
+__device__ __forceinline__ V3 center(const TriCam& c) { return V3{c.c[0], c.c[1], c.c[2]}; }
+__device__ __forceinline__ V3 center(const CahvCam& c) { return ld3(c.C); }
+template <bool ITER>
+__device__ __forceinline__ V3 ray(const TriCam& c, double u, double v, int* iters) { return pixel_to_vector<ITER>(c, u, v, iters); }
+template <bool ITER>
+__device__ __forceinline__ V3 ray(const CahvCam& c, double u, double v, int* iters) { return cahv_pixel_to_vector<ITER>(c, u, v, iters); }
+
+// StereoModel::operator()(pix1, pix2, errorVec) for two cameras of one family (StereoModel.cc:121-122 takes any camera's
+// pixel_to_vector and camera_center)
+template <bool ITER, class Cam>
+__device__ __forceinline__ V3 triangulate(const Cam& c0, const Cam& c1, double tol, double l0, double l1, double r0, double r1, V3* err,
+                                          int* iters) {
   *err = V3{0.0, 0.0, 0.0};
   const bool ok0 = !(l0 != l0 || l1 != l1) && !(l0 == -1e8 && l1 == -1e8);     // NaN or invalid_pixel(): the ray is skipped
   const bool ok1 = !(r0 != r0 || r1 != r1) && !(r0 == -1e8 && r1 == -1e8);
   if (!ok0 || !ok1) return V3{0.0, 0.0, 0.0};
-  const V3 d0 = pixel_to_vector<TSAI>(c0, l0, l1, iters), d1 = pixel_to_vector<TSAI>(c1, r0, r1, iters);
-  return intersect(V3{c0.c[0], c0.c[1], c0.c[2]}, V3{c1.c[0], c1.c[1], c1.c[2]}, d0, d1, tol, err);
-}
-
-// the same through CAHV / CAHVOR cameras (StereoModel.cc:121-122 takes any camera's pixel_to_vector and camera_center)
-__device__ __forceinline__ V3 triangulate_cahv(const CahvCam& c0, const CahvCam& c1, double tol, double l0, double l1, double r0, double r1,
-                                               V3* err, int* iters) {
-  *err = V3{0.0, 0.0, 0.0};
-  const bool ok0 = !(l0 != l0 || l1 != l1) && !(l0 == -1e8 && l1 == -1e8);
-  const bool ok1 = !(r0 != r0 || r1 != r1) && !(r0 == -1e8 && r1 == -1e8);
-  if (!ok0 || !ok1) return V3{0.0, 0.0, 0.0};
-  const V3 d0 = cahv_pixel_to_vector<true>(c0, l0, l1, iters), d1 = cahv_pixel_to_vector<true>(c1, r0, r1, iters);
-  return intersect(ld3(c0.C), ld3(c1.C), d0, d1, tol, err);
+  const V3 d0 = ray<ITER>(c0, l0, l1, iters), d1 = ray<ITER>(c1, r0, r1, iters);
+  return intersect(center(c0), center(c1), d0, d1, tol, err);
 }
 
 // the 32 {x, y, z} of a warp's consecutive pixels [0, n) to row + 3 * first, as three contiguous runs
@@ -71,7 +70,7 @@ template <class T> __device__ __forceinline__ double wide(const T& p, int i);
 template <> __device__ __forceinline__ double wide<vwb200_dispi>(const vwb200_dispi& p, int i) { return (double)(i ? p.dy : p.dx); }
 template <> __device__ __forceinline__ double wide<DispF>(const DispF& p, int i) { return (double)(i ? p.dy : p.dx); }
 
-// stats[0] error sum, [1] max error (bits), [2] points, [3] divergent, [4] Tsai Newton-Raphson iterations
+// stats[0] error sum, [1] max error (bits), [2] points, [3] divergent, [4] Newton iterations
 __device__ void flush_stats(unsigned long long* stats, double sum, double mx, unsigned long long pts, unsigned long long div, unsigned long long it) {
   for (int o = 16; o; o >>= 1) {
     sum = dadd(sum, __shfl_xor_sync(0xffffffffu, sum, o));
@@ -93,9 +92,10 @@ __device__ void flush_stats(unsigned long long* stats, double sum, double mx, un
 // MODEL == false: StereoView (form a) over the window (x0, y0, ow, oh): left pixel (i, j), right (i, j) + (double)disparity.
 // MODEL == true:  StereoModel::operator()(ImageView<PixelMask<Vector2f>>, error) (form b; x0 = y0 = 0): right pixel
 //                 (double)(x + d) summed in float, error = norm_2(errorVec), and the statistics the reference prints.
-template <class T, bool MODEL, bool TSAI>
+// ITER == false compiles the rays without their Newton iterations (kernel_for picks it per call).
+template <class Cam, class T, bool MODEL, bool ITER>
 __global__ void __launch_bounds__(kThreads, 4) k10_triangulate_kernel(const T* __restrict__ in, ptrdiff_t ip, int x0, int y0, int ow, int oh,
-                                                                   TriCam c0, TriCam c1, double tol, double* __restrict__ xyz, ptrdiff_t xp,
+                                                                   Cam c0, Cam c1, double tol, double* __restrict__ xyz, ptrdiff_t xp,
                                                                    double* __restrict__ err, ptrdiff_t ep, unsigned long long* stats) {
   __shared__ double stage[kWarps][96];
   const int first = blockIdx.x * kThreads + (threadIdx.x & ~31);                // the warp's first column
@@ -113,13 +113,13 @@ __global__ void __launch_bounds__(kThreads, 4) k10_triangulate_kernel(const T* _
         if (valid(d)) {
           const int x = x0 + i, y = y0 + j;
           if constexpr (MODEL) {
-            p = triangulate<TSAI>(c0, c1, tol, (double)x, (double)y, (double)__fadd_rn((float)x, chan(d, 0)),
+            p = triangulate<ITER>(c0, c1, tol, (double)x, (double)y, (double)__fadd_rn((float)x, chan(d, 0)),
                                   (double)__fadd_rn((float)y, chan(d, 1)), &e, &iters);
             error = norm3(e);
             if (error >= 0) { mx = fmax(mx, error); sum = dadd(sum, error); ++pts; }
             else { p = V3{0.0, 0.0, 0.0}; ++div; }                                 // rays diverged: NaN error
           } else {
-            p = triangulate<TSAI>(c0, c1, tol, (double)x, (double)y, dadd((double)x, wide(d, 0)), dadd((double)y, wide(d, 1)), &e, &iters);
+            p = triangulate<ITER>(c0, c1, tol, (double)x, (double)y, dadd((double)x, wide(d, 0)), dadd((double)y, wide(d, 1)), &e, &iters);
           }
         }
         if constexpr (MODEL) err[(ptrdiff_t)j * ep + i] = error;
@@ -127,53 +127,7 @@ __global__ void __launch_bounds__(kThreads, 4) k10_triangulate_kernel(const T* _
       store_xyz(stage[threadIdx.x >> 5], xyz + (ptrdiff_t)j * xp * 3 + 3 * (ptrdiff_t)first, n, p);
     }
   }
-  if (MODEL || TSAI) flush_stats(stats, sum, mx, pts, div, (unsigned long long)iters);
-}
-
-// a warp's sum of n added to *count
-__device__ __forceinline__ void flush_count(unsigned long long* count, unsigned long long n) {
-  for (int o = 16; o; o >>= 1) n += __shfl_xor_sync(0xffffffffu, n, o);
-  if ((threadIdx.x & 31) == 0 && n) atomicAdd(count, n);
-}
-
-// k10_triangulate_kernel's two forms through CAHV / CAHVOR cameras; stats[5] counts the CAHVOR Newton passes
-template <class T, bool MODEL>
-__global__ void __launch_bounds__(kThreads, 4) k10_triangulate_cahv_kernel(const T* __restrict__ in, ptrdiff_t ip, int x0, int y0, int ow, int oh,
-                                                                        const CahvCam c0, const CahvCam c1, double tol, double* __restrict__ xyz,
-                                                                        ptrdiff_t xp, double* __restrict__ err, ptrdiff_t ep,
-                                                                        unsigned long long* stats) {
-  __shared__ double stage[kWarps][96];
-  const int first = blockIdx.x * kThreads + (threadIdx.x & ~31);
-  const int n = min(32, ow - first);
-  const int i = blockIdx.x * kThreads + threadIdx.x;
-  double sum = 0.0, mx = 0.0;
-  unsigned long long pts = 0, div = 0;
-  int iters = 0;
-  if (n > 0) {
-    for (int j = blockIdx.y; j < oh; j += gridDim.y) {
-      V3 p{0.0, 0.0, 0.0}, e{0.0, 0.0, 0.0};
-      double error = 0.0;
-      if (i < ow) {
-        const T d = in[(ptrdiff_t)j * ip + i];
-        if (valid(d)) {
-          const int x = x0 + i, y = y0 + j;
-          if constexpr (MODEL) {
-            p = triangulate_cahv(c0, c1, tol, (double)x, (double)y, (double)__fadd_rn((float)x, chan(d, 0)), (double)__fadd_rn((float)y, chan(d, 1)),
-                                 &e, &iters);
-            error = norm3(e);
-            if (error >= 0) { mx = fmax(mx, error); sum = dadd(sum, error); ++pts; }
-            else { p = V3{0.0, 0.0, 0.0}; ++div; }
-          } else {
-            p = triangulate_cahv(c0, c1, tol, (double)x, (double)y, dadd((double)x, wide(d, 0)), dadd((double)y, wide(d, 1)), &e, &iters);
-          }
-        }
-        if constexpr (MODEL) err[(ptrdiff_t)j * ep + i] = error;
-      }
-      store_xyz(stage[threadIdx.x >> 5], xyz + (ptrdiff_t)j * xp * 3 + 3 * (ptrdiff_t)first, n, p);
-    }
-  }
-  if (MODEL) flush_stats(stats, sum, mx, pts, div, 0);
-  flush_count(stats + 5, (unsigned long long)iters);
+  if (MODEL || ITER) flush_stats(stats, sum, mx, pts, div, (unsigned long long)iters);
 }
 
 // UniverseRadiusFunc::operator()(Vector3) (StereoView.h:172-186) over a w x h Vector3 image; in may be out (same pitch).
@@ -215,53 +169,44 @@ dim3 grid_for(int w, int h) {
   return dim3(gx, gy);
 }
 
+// the kernel for a camera pair: a pinhole pair's iterates when either camera has the Tsai lens, a CAHV pair's always (whether
+// a camera is CAHVOR is a runtime flag)
+template <class T, bool MODEL>
+auto kernel_for(const TriCam& c0, const TriCam& c1) {
+  return c0.tsai || c1.tsai ? k10_triangulate_kernel<TriCam, T, MODEL, true> : k10_triangulate_kernel<TriCam, T, MODEL, false>;
+}
+template <class T, bool MODEL>
+auto kernel_for(const CahvCam&, const CahvCam&) { return k10_triangulate_kernel<CahvCam, T, MODEL, true>; }
+
 }  // namespace
 
-template <class T>
-int stereo_triangulate_launch(const T* in, ptrdiff_t ip, int x0, int y0, int ow, int oh, const TriCam& c0, const TriCam& c1, double tol,
+template <class Cam, class T>
+int stereo_triangulate_launch(const T* in, ptrdiff_t ip, int x0, int y0, int ow, int oh, const Cam& c0, const Cam& c1, double tol,
                               double* xyz, ptrdiff_t xp, unsigned long long* stats, cudaStream_t st) {
-  const dim3 g = grid_for(ow, oh);
-  if (c0.tsai || c1.tsai)
-    k10_triangulate_kernel<T, false, true><<<g, kThreads, 0, st>>>(in, ip, x0, y0, ow, oh, c0, c1, tol, xyz, xp, nullptr, 0, stats);
-  else
-    k10_triangulate_kernel<T, false, false><<<g, kThreads, 0, st>>>(in, ip, x0, y0, ow, oh, c0, c1, tol, xyz, xp, nullptr, 0, stats);
+  kernel_for<T, false>(c0, c1)<<<grid_for(ow, oh), kThreads, 0, st>>>(in, ip, x0, y0, ow, oh, c0, c1, tol, xyz, xp, nullptr, 0, stats);
   VWB_LAUNCH_CHECK();
   return VWB200_OK;
 }
-template int stereo_triangulate_launch<vwb200_dispi>(const vwb200_dispi*, ptrdiff_t, int, int, int, int, const TriCam&, const TriCam&, double,
-                                                     double*, ptrdiff_t, unsigned long long*, cudaStream_t);
-template int stereo_triangulate_launch<DispF>(const DispF*, ptrdiff_t, int, int, int, int, const TriCam&, const TriCam&, double, double*,
-                                              ptrdiff_t, unsigned long long*, cudaStream_t);
+template int stereo_triangulate_launch<TriCam, vwb200_dispi>(const vwb200_dispi*, ptrdiff_t, int, int, int, int, const TriCam&, const TriCam&,
+                                                             double, double*, ptrdiff_t, unsigned long long*, cudaStream_t);
+template int stereo_triangulate_launch<TriCam, DispF>(const DispF*, ptrdiff_t, int, int, int, int, const TriCam&, const TriCam&, double, double*,
+                                                      ptrdiff_t, unsigned long long*, cudaStream_t);
+template int stereo_triangulate_launch<CahvCam, vwb200_dispi>(const vwb200_dispi*, ptrdiff_t, int, int, int, int, const CahvCam&, const CahvCam&,
+                                                              double, double*, ptrdiff_t, unsigned long long*, cudaStream_t);
+template int stereo_triangulate_launch<CahvCam, DispF>(const DispF*, ptrdiff_t, int, int, int, int, const CahvCam&, const CahvCam&, double,
+                                                       double*, ptrdiff_t, unsigned long long*, cudaStream_t);
 
-int stereo_model_launch(const DispF* in, int w, int h, ptrdiff_t ip, const TriCam& c0, const TriCam& c1, double tol, double* xyz, ptrdiff_t xp,
+template <class Cam>
+int stereo_model_launch(const DispF* in, int w, int h, ptrdiff_t ip, const Cam& c0, const Cam& c1, double tol, double* xyz, ptrdiff_t xp,
                         double* err, ptrdiff_t ep, unsigned long long* stats, cudaStream_t st) {
-  const dim3 g = grid_for(w, h);
-  if (c0.tsai || c1.tsai)
-    k10_triangulate_kernel<DispF, true, true><<<g, kThreads, 0, st>>>(in, ip, 0, 0, w, h, c0, c1, tol, xyz, xp, err, ep, stats);
-  else
-    k10_triangulate_kernel<DispF, true, false><<<g, kThreads, 0, st>>>(in, ip, 0, 0, w, h, c0, c1, tol, xyz, xp, err, ep, stats);
+  kernel_for<DispF, true>(c0, c1)<<<grid_for(w, h), kThreads, 0, st>>>(in, ip, 0, 0, w, h, c0, c1, tol, xyz, xp, err, ep, stats);
   VWB_LAUNCH_CHECK();
   return VWB200_OK;
 }
-
-template <class T>
-int cahv_stereo_triangulate_launch(const T* in, ptrdiff_t ip, int x0, int y0, int ow, int oh, const CahvCam& c0, const CahvCam& c1, double tol,
-                                   double* xyz, ptrdiff_t xp, unsigned long long* stats, cudaStream_t st) {
-  k10_triangulate_cahv_kernel<T, false><<<grid_for(ow, oh), kThreads, 0, st>>>(in, ip, x0, y0, ow, oh, c0, c1, tol, xyz, xp, nullptr, 0, stats);
-  VWB_LAUNCH_CHECK();
-  return VWB200_OK;
-}
-template int cahv_stereo_triangulate_launch<vwb200_dispi>(const vwb200_dispi*, ptrdiff_t, int, int, int, int, const CahvCam&, const CahvCam&,
-                                                          double, double*, ptrdiff_t, unsigned long long*, cudaStream_t);
-template int cahv_stereo_triangulate_launch<DispF>(const DispF*, ptrdiff_t, int, int, int, int, const CahvCam&, const CahvCam&, double, double*,
-                                                   ptrdiff_t, unsigned long long*, cudaStream_t);
-
-int cahv_stereo_model_launch(const DispF* in, int w, int h, ptrdiff_t ip, const CahvCam& c0, const CahvCam& c1, double tol, double* xyz,
-                             ptrdiff_t xp, double* err, ptrdiff_t ep, unsigned long long* stats, cudaStream_t st) {
-  k10_triangulate_cahv_kernel<DispF, true><<<grid_for(w, h), kThreads, 0, st>>>(in, ip, 0, 0, w, h, c0, c1, tol, xyz, xp, err, ep, stats);
-  VWB_LAUNCH_CHECK();
-  return VWB200_OK;
-}
+template int stereo_model_launch<TriCam>(const DispF*, int, int, ptrdiff_t, const TriCam&, const TriCam&, double, double*, ptrdiff_t, double*,
+                                         ptrdiff_t, unsigned long long*, cudaStream_t);
+template int stereo_model_launch<CahvCam>(const DispF*, int, int, ptrdiff_t, const CahvCam&, const CahvCam&, double, double*, ptrdiff_t, double*,
+                                          ptrdiff_t, unsigned long long*, cudaStream_t);
 
 int universe_radius_launch(const double* in, int w, int h, ptrdiff_t ip, const double* origin, double near_r, double far_r, double* out,
                            ptrdiff_t op, unsigned long long* rejected, cudaStream_t st) {

@@ -11,6 +11,7 @@
 // resize_epipolar_cameras_to_fit through the same cameras.  The internal kinds kCahv and kCahvMasked are the same transform
 // from a CAHV or CAHVOR src into a CAHV dst, through cahv.cuh (the src model is a runtime branch on its flag; the dst is CAHV
 // at compile time, so the CAHVOR Newton loop is not compiled in; the CAHV family has no point_to_pixel check).
+#include <type_traits>
 #include "cahv.cuh"
 
 namespace vwb200 {
@@ -235,25 +236,23 @@ __global__ void __launch_bounds__(128) k8_camera_bbox_kernel(const TriCam src, c
 
 }  // namespace
 
-int camera_warp_launch(int masked, int interp, int edge, const float* edge_value, const TriCam& src, const TriCam& dst, const float* in, int w,
-                       int h, ptrdiff_t ip, int x0, int y0, float* out, int ow, int oh, ptrdiff_t op, unsigned long long* fail, cudaStream_t st) {
+template <class Cam>
+int camera_warp_launch(int masked, int interp, int edge, const float* edge_value, const Cam& src, const Cam& dst, const float* in, int w, int h,
+                       ptrdiff_t ip, int x0, int y0, float* out, int ow, int oh, ptrdiff_t op, unsigned long long* fail, cudaStream_t st) {
   if (ow <= 0 || oh <= 0) return VWB200_OK;
-  WarpArgs a{in, w, h, ip, nullptr, 0, 0, 0, {}, x0, y0, out, ow, oh, op, src, dst, fail, make_float2(edge_value[0], edge_value[1])};
-  if (!masked) return launch_interp<kCamera>(interp, edge, a, st);
-  if (edge == VWB200_EDGE_ZERO) return launch<kCameraMasked, VWB200_INTERP_BILINEAR, VWB200_EDGE_ZERO>(a, st);
-  if (edge == VWB200_EDGE_CONSTANT) return launch<kCameraMasked, VWB200_INTERP_BILINEAR, VWB200_EDGE_CONSTANT>(a, st);
-  return launch<kCameraMasked, VWB200_INTERP_BILINEAR, VWB200_EDGE_VALUE>(a, st);
+  WarpArgs a{in, w, h, ip, nullptr, 0, 0, 0, {}, x0, y0, out, ow, oh, op, {}, {}, fail, make_float2(edge_value[0], edge_value[1])};
+  constexpr bool cahv = std::is_same<Cam, CahvCam>::value;
+  if constexpr (cahv) { a.csrc = src; a.cdst = dst; } else { a.src = src; a.dst = dst; }
+  constexpr int kind = cahv ? kCahv : kCamera, masked_kind = cahv ? kCahvMasked : kCameraMasked;
+  if (!masked) return launch_interp<kind>(interp, edge, a, st);
+  if (edge == VWB200_EDGE_ZERO) return launch<masked_kind, VWB200_INTERP_BILINEAR, VWB200_EDGE_ZERO>(a, st);
+  if (edge == VWB200_EDGE_CONSTANT) return launch<masked_kind, VWB200_INTERP_BILINEAR, VWB200_EDGE_CONSTANT>(a, st);
+  return launch<masked_kind, VWB200_INTERP_BILINEAR, VWB200_EDGE_VALUE>(a, st);
 }
-
-int cahv_warp_launch(int masked, int interp, int edge, const float* edge_value, const CahvCam& src, const CahvCam& dst, const float* in, int w,
-                     int h, ptrdiff_t ip, int x0, int y0, float* out, int ow, int oh, ptrdiff_t op, cudaStream_t st) {
-  if (ow <= 0 || oh <= 0) return VWB200_OK;
-  WarpArgs a{in, w, h, ip, nullptr, 0, 0, 0, {}, x0, y0, out, ow, oh, op, {}, {}, nullptr, make_float2(edge_value[0], edge_value[1]), src, dst};
-  if (!masked) return launch_interp<kCahv>(interp, edge, a, st);
-  if (edge == VWB200_EDGE_ZERO) return launch<kCahvMasked, VWB200_INTERP_BILINEAR, VWB200_EDGE_ZERO>(a, st);
-  if (edge == VWB200_EDGE_CONSTANT) return launch<kCahvMasked, VWB200_INTERP_BILINEAR, VWB200_EDGE_CONSTANT>(a, st);
-  return launch<kCahvMasked, VWB200_INTERP_BILINEAR, VWB200_EDGE_VALUE>(a, st);
-}
+template int camera_warp_launch<TriCam>(int, int, int, const float*, const TriCam&, const TriCam&, const float*, int, int, ptrdiff_t, int, int,
+                                        float*, int, int, ptrdiff_t, unsigned long long*, cudaStream_t);
+template int camera_warp_launch<CahvCam>(int, int, int, const float*, const CahvCam&, const CahvCam&, const float*, int, int, ptrdiff_t, int, int,
+                                         float*, int, int, ptrdiff_t, unsigned long long*, cudaStream_t);
 
 int camera_bbox_launch(const TriCam& src, const TriCam& dst, int x0, int y0, int x1, int y1, unsigned* keys4, unsigned long long* fail,
                        cudaStream_t st) {
