@@ -3,7 +3,8 @@
 // Newton loop on k5*u^5 + k3*u^3 + k1*u = 1) and point_to_pixel (CAHVModel.cc:167-171; CAHVORModel.cc:431-448).  Neither
 // has a round-trip check.  The camera is a CahvCam; cahvor == 0 is a CAHV camera.  As in pinhole.cuh every product, sum,
 // quotient and square root is an explicitly rounded intrinsic in the reference's order (dot products and norms summed from
-// 0.0, normalize dividing each component by norm_2), so nothing is contracted into an FMA.
+// 0.0, normalize dividing each component by norm_2), so nothing is contracted into an FMA.  The vector helpers and
+// cahv_pixel_to_vector are also the host's: linearize_camera (cameras.cu) evaluates the CAHVOR rays with them.
 #pragma once
 #include "pinhole.cuh"
 
@@ -13,10 +14,9 @@ namespace {
 constexpr int kCahvorMaxIter = 20;                     // VW_CAHVOR_MAXITER (CAHVORModel.cc:115)
 constexpr double kCahvorConv = 1.0e-6;                 // VW_CAHVOR_CONV (:116)
 
-__device__ __forceinline__ V3 ld3(const double* p) { return V3{p[0], p[1], p[2]}; }
-__device__ __forceinline__ V3 add3(V3 a, V3 b) { return V3{dadd(a.x, b.x), dadd(a.y, b.y), dadd(a.z, b.z)}; }
-__device__ __forceinline__ V3 scale3(double s, V3 a) { return V3{dmul(s, a.x), dmul(s, a.y), dmul(s, a.z)}; }
-__device__ __forceinline__ V3 normalize3(V3 a) {       // Math/Vector.h:1694: each component / norm_2
+__host__ __device__ __forceinline__ V3 add3(V3 a, V3 b) { return V3{dadd(a.x, b.x), dadd(a.y, b.y), dadd(a.z, b.z)}; }
+__host__ __device__ __forceinline__ V3 scale3(double s, V3 a) { return V3{dmul(s, a.x), dmul(s, a.y), dmul(s, a.z)}; }
+__host__ __device__ __forceinline__ V3 normalize3(V3 a) {  // Math/Vector.h:1694: each component / norm_2
   const double n = norm3(a);
   return V3{ddiv(a.x, n), ddiv(a.y, n), ddiv(a.z, n)};
 }
@@ -25,7 +25,7 @@ __device__ __forceinline__ V3 normalize3(V3 a) {       // Math/Vector.h:1694: ea
 // distortion removed by Newton's method.  *iters counts the Newton passes (each computes poly and deriv).  MAYBE_CAHVOR ==
 // false compiles the CAHV form alone, for a camera the host has checked to be CAHV (camera_transform's destination).
 template <bool MAYBE_CAHVOR>
-__device__ __forceinline__ V3 cahv_pixel_to_vector(const CahvCam& c, double x, double y, int* iters) {
+__host__ __device__ __forceinline__ V3 cahv_pixel_to_vector(const CahvCam& c, double x, double y, int* iters) {
   const V3 A = ld3(c.A);
   V3 rr = normalize3(cross3(sub3(ld3(c.V), scale3(y, A)), sub3(ld3(c.H), scale3(x, A))));
   if (c.flip) rr = scale3(-1.0, rr);

@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stddef.h>
+#include <cstring>
 #include <string>
 #include <atomic>
 #include <vector>
@@ -61,14 +62,98 @@ struct Arena {
   }
 };
 
-// ---- order-preserving keys of floats (median select, outlier cutoff) -----------------------------
+// an owned-or-borrowed stream
+struct StreamGuard {
+  cudaStream_t st = nullptr; bool own = false;
+  // device-resident inputs are produced on the caller's stream: a NULL stream then means the legacy default stream
+  // (which is what e.g. torch's default stream is), never a private one -- otherwise the kernels could start before the
+  // producer of their inputs has finished.  Host-resident calls with no stream get a private non-blocking stream.
+  int init(void* user, int device_resident = 0) {
+    if (user) { st = static_cast<cudaStream_t>(user); return VWB200_OK; }
+    if (device_resident) { st = cudaStreamLegacy; return VWB200_OK; }
+    VWB_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+    own = true;
+    return VWB200_OK;
+  }
+  ~StreamGuard() { if (own && st) cudaStreamDestroy(st); }
+};
+
+// One call of the C ABI: its stream, its stream-ordered scratch, and the moves of the caller's rasters between the host and
+// HBM.  Widths and pitches count elements of T (a float triple is 3 floats, a search box 4 int32).  finish() copies the
+// staged outputs back and synchronises the stream: every call returns with its work done, device-resident calls included.
+struct AbiCall {
+  StreamGuard sg;
+  Arena ar{nullptr};
+  cudaStream_t st = nullptr;
+  struct CopyBack { void* dst; size_t dpitch; const void* src; size_t row; int h; cudaMemcpyKind kind; const int* unless; };
+  std::vector<CopyBack> backs;
+
+  int open(void* stream, int device_resident) {
+    VWB_TRY(sg.init(stream, device_resident));
+    st = ar.st = sg.st;
+    return VWB200_OK;
+  }
+  // an input: the caller's device raster, or a dense HBM copy of the host raster
+  template <class T> int in(const T* src, int w, int h, ptrdiff_t pitch, int on_device, const T** dev, ptrdiff_t* dpitch) {
+    if (on_device) { *dev = src; *dpitch = pitch; return VWB200_OK; }
+    T* d;
+    VWB_TRY(ar.alloc(&d, (size_t)w * h));
+    VWB_CUDA(cudaMemcpy2DAsync(d, (size_t)w * sizeof(T), src, (size_t)pitch * sizeof(T), (size_t)w * sizeof(T), h, cudaMemcpyHostToDevice, st));
+    *dev = d; *dpitch = w;
+    return VWB200_OK;
+  }
+  // an output `user` (may be NULL: scratch only): the caller's device raster itself -- when `dense` asks for it, only if its
+  // pitch is w -- or a dense HBM buffer that finish() copies to `user`, w elements per row so that the pitch padding is never
+  // written, unless *unless is set by then.  The buffer starts as a copy of `init` (an in-out raster passes itself), which
+  // lives where the call's inputs live.
+  template <class T> int out(T* user, int w, int h, ptrdiff_t pitch, int on_device, T** dev, ptrdiff_t* dpitch, const T* init = nullptr,
+                             ptrdiff_t ipitch = 0, bool dense = false, const int* unless = nullptr) {
+    if (on_device && user && (!init || init == user) && (!dense || pitch == w)) { *dev = user; *dpitch = pitch; return VWB200_OK; }
+    VWB_TRY(ar.alloc(dev, (size_t)w * h));
+    *dpitch = w;
+    const size_t row = (size_t)w * sizeof(T);
+    if (init)
+      VWB_CUDA(cudaMemcpy2DAsync(*dev, row, init, (size_t)ipitch * sizeof(T), row, h, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
+    if (user) backs.push_back(CopyBack{user, (size_t)pitch * sizeof(T), *dev, row, h, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, unless});
+    return VWB200_OK;
+  }
+  int finish() {
+    for (const CopyBack& b : backs)
+      if (!b.unless || !*b.unless) VWB_CUDA(cudaMemcpy2DAsync(b.dst, b.dpitch, b.src, b.row, b.row, b.h, b.kind, st));
+    VWB_CUDA(cudaStreamSynchronize(st));
+    return VWB200_OK;
+  }
+};
+
+// [a0, a1) and [b0, b1): the bytes of an w x h / ow x oh raster of `apx` / `bpx`-byte pixels (disparity pixels by default)
+inline bool rasters_overlap(const void* a, int w, int h, ptrdiff_t ap, const void* b, int ow, int oh, ptrdiff_t bp, size_t apx = 12,
+                            size_t bpx = 12) {
+  if (w <= 0 || h <= 0 || ow <= 0 || oh <= 0) return false;
+  const uintptr_t a0 = (uintptr_t)a, a1 = a0 + ((size_t)(h - 1) * ap + w) * apx;
+  const uintptr_t b0 = (uintptr_t)b, b1 = b0 + ((size_t)(oh - 1) * bp + ow) * bpx;
+  return a0 < b1 && b0 < a1;
+}
+
+// ---- order-preserving keys of floats (median select, outlier cutoff, bounding boxes) -----------------------------
 // -0.0 sorts just below +0.0; NaN is outside the contract
-__device__ __forceinline__ unsigned fkey(float f) {
-  unsigned u = __float_as_uint(f);
+__host__ __device__ __forceinline__ unsigned fkey(float f) {
+#ifdef __CUDA_ARCH__
+  const unsigned u = __float_as_uint(f);
+#else
+  unsigned u;
+  std::memcpy(&u, &f, sizeof u);
+#endif
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
-__device__ __forceinline__ float kfloat(unsigned k) {
-  return __uint_as_float((k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k);
+__host__ __device__ __forceinline__ float kfloat(unsigned k) {
+  const unsigned u = (k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k;
+#ifdef __CUDA_ARCH__
+  return __uint_as_float(u);
+#else
+  float f;
+  std::memcpy(&f, &u, sizeof f);
+  return f;
+#endif
 }
 
 // ---- image descriptors (device pointers) ------------------------------------------------------

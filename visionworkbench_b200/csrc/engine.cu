@@ -1,5 +1,5 @@
 // engine.cu -- host side of the vwb200 engine: error plumbing, the extern "C" ABI of
-// include/vwb200.h, and the per-tile level loop of PyramidCorrelationView::prerasterize
+// include/vwb200.h (its camera calls are in cameras.cu), and the per-tile level loop of PyramidCorrelationView::prerasterize
 // (behaviour of Stereo/CorrelationView.cc:273-886, block-matching branch) driving the CUDA kernels.
 //
 // Everything here is re-entrant: no mutable globals except the launch counter; each rasterize call
@@ -60,24 +60,6 @@ int ensure_device() {
 int zone_post_launch(const Tile* d_tiles, int ntiles, const Zone* d_zones, const Zone* d_rlzones, const int2* d_post_add,
                      vwb200_dispi* disp, const vwb200_dispi* rl, float thr, int tile_w, int tile_h, cudaStream_t st, float* diff = nullptr,
                      ptrdiff_t dpitch = 0, int dox = 0, int doy = 0);
-
-// ---------------------------------------------------------------------------------------------------
-// small RAII helpers: stream-ordered device buffers, an owned-or-borrowed stream
-// ---------------------------------------------------------------------------------------------------
-struct StreamGuard {
-  cudaStream_t st = nullptr; bool own = false;
-  // device-resident inputs are produced on the caller's stream: a NULL stream then means the legacy default stream
-  // (which is what e.g. torch's default stream is), never a private one -- otherwise the kernels could start before the
-  // producer of their inputs has finished.  Host-resident calls with no stream get a private non-blocking stream.
-  int init(void* user, int device_resident = 0) {
-    if (user) { st = static_cast<cudaStream_t>(user); return VWB200_OK; }
-    if (device_resident) { st = cudaStreamLegacy; return VWB200_OK; }
-    VWB_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-    own = true;
-    return VWB200_OK;
-  }
-  ~StreamGuard() { if (own && st) cudaStreamDestroy(st); }
-};
 
 static void make_tiles(const std::vector<Zone>& zones, int tile_w, int tile_h, std::vector<Tile>& tiles, bool with_chunks) {
   tiles.clear();
@@ -883,53 +865,6 @@ int vwb200_corr::prerasterize_sgm(Box bbox, const std::vector<LevelImgs>& py, in
   return VWB200_OK;
 }
 
-// One call of the C ABI: its stream, its stream-ordered scratch, and the moves of the caller's rasters between the host and
-// HBM.  Widths and pitches count elements of T (a float triple is 3 floats, a search box 4 int32).  finish() copies the
-// staged outputs back and synchronises the stream: every call returns with its work done, device-resident calls included.
-struct AbiCall {
-  StreamGuard sg;
-  Arena ar{nullptr};
-  cudaStream_t st = nullptr;
-  struct CopyBack { void* dst; size_t dpitch; const void* src; size_t row; int h; cudaMemcpyKind kind; const int* unless; };
-  std::vector<CopyBack> backs;
-
-  int open(void* stream, int device_resident) {
-    VWB_TRY(sg.init(stream, device_resident));
-    st = ar.st = sg.st;
-    return VWB200_OK;
-  }
-  // an input: the caller's device raster, or a dense HBM copy of the host raster
-  template <class T> int in(const T* src, int w, int h, ptrdiff_t pitch, int on_device, const T** dev, ptrdiff_t* dpitch) {
-    if (on_device) { *dev = src; *dpitch = pitch; return VWB200_OK; }
-    T* d;
-    VWB_TRY(ar.alloc(&d, (size_t)w * h));
-    VWB_CUDA(cudaMemcpy2DAsync(d, (size_t)w * sizeof(T), src, (size_t)pitch * sizeof(T), (size_t)w * sizeof(T), h, cudaMemcpyHostToDevice, st));
-    *dev = d; *dpitch = w;
-    return VWB200_OK;
-  }
-  // an output `user` (may be NULL: scratch only): the caller's device raster itself -- when `dense` asks for it, only if its
-  // pitch is w -- or a dense HBM buffer that finish() copies to `user`, w elements per row so that the pitch padding is never
-  // written, unless *unless is set by then.  The buffer starts as a copy of `init` (an in-out raster passes itself), which
-  // lives where the call's inputs live.
-  template <class T> int out(T* user, int w, int h, ptrdiff_t pitch, int on_device, T** dev, ptrdiff_t* dpitch, const T* init = nullptr,
-                             ptrdiff_t ipitch = 0, bool dense = false, const int* unless = nullptr) {
-    if (on_device && user && (!init || init == user) && (!dense || pitch == w)) { *dev = user; *dpitch = pitch; return VWB200_OK; }
-    VWB_TRY(ar.alloc(dev, (size_t)w * h));
-    *dpitch = w;
-    const size_t row = (size_t)w * sizeof(T);
-    if (init)
-      VWB_CUDA(cudaMemcpy2DAsync(*dev, row, init, (size_t)ipitch * sizeof(T), row, h, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
-    if (user) backs.push_back(CopyBack{user, (size_t)pitch * sizeof(T), *dev, row, h, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, unless});
-    return VWB200_OK;
-  }
-  int finish() {
-    for (const CopyBack& b : backs)
-      if (!b.unless || !*b.unless) VWB_CUDA(cudaMemcpy2DAsync(b.dst, b.dpitch, b.src, b.row, b.row, b.h, b.kind, st));
-    VWB_CUDA(cudaStreamSynchronize(st));
-    return VWB200_OK;
-  }
-};
-
 // one outlier filter call: the input staged or used in place, the output written densely and copied back
 template <class T>
 static int outlier_filter_typed(const vwb200_outlier_params& p, const T* in, int w, int h, ptrdiff_t pitch, T* out, ptrdiff_t opitch,
@@ -970,14 +905,6 @@ static int dispmap_check(const char* what, int pixel_type, const void* in, int w
   if (pixel_type != VWB200_DISP_I32 && pixel_type != VWB200_DISP_F32) { set_error("%s: unknown pixel type %d", what, pixel_type); return VWB200_EARG; }
   if (w < 0 || h < 0 || pitch < w) { set_error("%s: bad size %d x %d, pitch %td", what, w, h, pitch); return VWB200_EARG; }
   return VWB200_OK;
-}
-// [a0, a1) and [b0, b1): the bytes of an w x h / ow x oh raster of `apx` / `bpx`-byte pixels (disparity pixels by default)
-static bool rasters_overlap(const void* a, int w, int h, ptrdiff_t ap, const void* b, int ow, int oh, ptrdiff_t bp, size_t apx = 12,
-                            size_t bpx = 12) {
-  if (w <= 0 || h <= 0 || ow <= 0 || oh <= 0) return false;
-  const uintptr_t a0 = (uintptr_t)a, a1 = a0 + ((size_t)(h - 1) * ap + w) * apx;
-  const uintptr_t b0 = (uintptr_t)b, b1 = b0 + ((size_t)(oh - 1) * bp + ow) * bpx;
-  return a0 < b1 && b0 < a1;
 }
 // one resampling or per-pixel call: in (w x h) -> out (ow x oh), both staged through AbiCall.  launch(din, dp, dout, dop, st)
 // is called with device pointers of the pixel type; out == in on the device (same pitch) is used in place.
@@ -1794,774 +1721,7 @@ int vwb200_remove_duplicate_matches(const float* xy1, const float* xy2, int n, i
   return VWB200_OK;
 }
 
-// ---- K10: triangulation (Stereo/StereoView.h, StereoModel.cc) through pinhole cameras ------------------------------------------
-// The camera is built on the host once per call, in the reference's operation order (x86-64 host code has no FMA to contract
-// into, so every product and sum rounds as the reference's does).
-struct Pt3 { double x, y, z; };
-static thread_local vwb200_triangulation_stats t_tri_stats = {0, 0, 0.0, 0.0, 0};
-
-static double dot3h(const double* a, const double* b) { double r = 0.0; for (int k = 0; k < 3; ++k) r += a[k] * b[k]; return r; }
-
-// vw::math::inverse (Math/Matrix.h:2218-2281) of a 3 x 3 matrix: LU with partial pivoting (the first largest |pivot|), then
-// the lower and upper triangular solves on the permuted identity, in its loop order
-static int lu_inverse3(const double* m, double* inv) {
-  double b[9];
-  std::memcpy(b, m, sizeof b);
-  int pm[3] = {0, 1, 2};
-  for (int i = 0; i < 3; ++i) {
-    int p = i;
-    double mx = -1;
-    for (int k = i; k < 3; ++k)
-      if (std::fabs(b[3 * k + i]) > mx) { mx = std::fabs(b[3 * k + i]); p = k; }
-    if (b[3 * p + i] == 0.0) { set_error("Matrix is singular in inverse()"); return VWB200_EMATH; }
-    if (p != i) {
-      std::swap(pm[i], pm[p]);
-      for (int c = 0; c < 3; ++c) std::swap(b[3 * i + c], b[3 * p + c]);
-    }
-    if (i != 2) {
-      for (int k = i + 1; k < 3; ++k) b[3 * k + i] /= b[3 * i + i];
-      for (int k = i + 1; k < 3; ++k)
-        for (int c = i + 1; c < 3; ++c) b[3 * k + c] -= b[3 * k + i] * b[3 * i + c];
-    }
-  }
-  for (int k = 0; k < 9; ++k) inv[k] = 0.0;
-  for (int i = 0; i < 3; ++i) inv[3 * i + pm[i]] = 1.0;
-  for (int i = 0; i < 3; ++i)
-    for (int j = 0; j < 3; ++j) {
-      const double t = inv[3 * i + j];
-      if (t != 0.0)
-        for (int k = i + 1; k < 3; ++k) inv[3 * k + j] -= b[3 * k + i] * t;
-    }
-  for (int i = 2; i >= 0; --i)
-    for (int j = 2; j >= 0; --j) {
-      const double t = inv[3 * i + j] /= b[3 * i + i];
-      if (t != 0.0)
-        for (int k = i - 1; k >= 0; --k) inv[3 * k + j] -= b[3 * k + i] * t;
-    }
-  return VWB200_OK;
-}
-
-// the argument checks of one camera (VWB200_EARG)
-static int pinhole_check(const char* what, const vwb200_pinhole* p) {
-  if (!p) { set_error("%s: null camera", what); return VWB200_EARG; }
-  if (p->lens != VWB200_LENS_NULL && p->lens != VWB200_LENS_TSAI) { set_error("%s: unknown lens distortion %d", what, p->lens); return VWB200_EARG; }
-  const int want = p->lens == VWB200_LENS_TSAI ? 5 : 0;
-  if (p->num_lens_params != want) {
-    set_error("%s: the %s lens distortion takes %d parameters, not %d", what, want ? "TSAI" : "NULL", want, p->num_lens_params);
-    return VWB200_EARG;
-  }
-  return VWB200_OK;
-}
-
-// PinholeModel::rebuild_camera_matrix (PinholeModel.cc:553-605): the orthonormality asserts of u, v, w (VW_LINE_ASSERT throws
-// LogicErr), then m_inv_camera_transform = inverse(uvw * transpose(R)) * inverse(K), each product a dot_prod from 0.0
-static int pinhole_build(const char* what, const vwb200_pinhole& p, TriCam* c) {
-  const double* uvw[3] = {p.u_direction, p.v_direction, p.w_direction};
-  const bool ortho = dot3h(uvw[0], uvw[1]) == 0 && dot3h(uvw[0], uvw[2]) == 0 && dot3h(uvw[1], uvw[2]) == 0 &&
-                     std::fabs(std::sqrt(dot3h(uvw[0], uvw[0])) - 1) < 0.001 && std::fabs(std::sqrt(dot3h(uvw[1], uvw[1])) - 1) < 0.001 &&
-                     std::fabs(std::sqrt(dot3h(uvw[2], uvw[2])) - 1) < 0.001;
-  if (!ortho) { set_error("%s: the u, v, w coordinate frame is not orthonormal", what); return VWB200_ELOGIC; }
-  double m[9], k[9] = {p.fu, 0, p.cu, 0, p.fv, p.cv, 0, 0, 1}, a[9], b[9];
-  for (int i = 0; i < 3; ++i)
-    for (int j = 0; j < 3; ++j) m[3 * i + j] = dot3h(uvw[i], p.rotation + 3 * j);       // row i of uvw . column j of R^T
-  VWB_TRY(lu_inverse3(m, a));
-  VWB_TRY(lu_inverse3(k, b));
-  for (int i = 0; i < 3; ++i)
-    for (int j = 0; j < 3; ++j) {
-      double r = 0.0;
-      for (int q = 0; q < 3; ++q) r += a[3 * i + q] * b[3 * q + j];
-      c->inv[3 * i + j] = r;
-    }
-  for (int q = 0; q < 3; ++q) c->c[q] = p.center[q];
-  c->pitch = p.pixel_pitch;
-  c->fu = p.fu; c->fv = p.fv; c->cu = p.cu; c->cv = p.cv;
-  for (int q = 0; q < 5; ++q) c->k[q] = p.lens == VWB200_LENS_TSAI ? p.lens_params[q] : 0.0;
-  c->tsai = p.lens == VWB200_LENS_TSAI;
-  // m_camera_matrix = K * [uvw * transpose(R) | (uvw * (-transpose(R))) * C], every element a dot_prod from 0.0
-  double e[12];
-  for (int i = 0; i < 3; ++i) {
-    double m2[3];
-    for (int j = 0; j < 3; ++j) {
-      e[4 * i + j] = m[3 * i + j];
-      const double nr[3] = {-p.rotation[3 * j], -p.rotation[3 * j + 1], -p.rotation[3 * j + 2]};
-      m2[j] = dot3h(uvw[i], nr);
-    }
-    e[4 * i + 3] = dot3h(m2, p.center);
-  }
-  for (int i = 0; i < 3; ++i)
-    for (int j = 0; j < 4; ++j) {
-      double r = 0.0;
-      for (int q = 0; q < 3; ++q) r += k[3 * i + q] * e[4 * q + j];
-      c->P[4 * i + j] = r;
-    }
-  return VWB200_OK;
-}
-
-// the five zeroed device statistics of one call
-static int tri_stats_open(AbiCall& c, unsigned long long** d) {
-  VWB_TRY(c.ar.alloc(d, 5));
-  VWB_CUDA(cudaMemsetAsync(*d, 0, 5 * sizeof(unsigned long long), c.st));
-  return VWB200_OK;
-}
-
-int vwb200_last_triangulation_stats(vwb200_triangulation_stats* out) { if (!out) return VWB200_EARG; *out = t_tri_stats; return VWB200_OK; }
-
-// the raster checks of stereo_triangulate (after the cameras')
-static int triangulate_args(const char* what, const void* disparity, int w, int h, ptrdiff_t pitch, int x0, int y0, int ow, int oh,
-                            const double* xyz, ptrdiff_t xyz_pitch) {
-  if (w <= 0 || h <= 0 || pitch < w) { set_error("%s: bad input size %d x %d, pitch %td", what, w, h, pitch); return VWB200_EARG; }
-  if (ow <= 0 || oh <= 0 || xyz_pitch < ow) { set_error("%s: bad output size %d x %d, pitch %td", what, ow, oh, xyz_pitch); return VWB200_EARG; }
-  if (x0 < 0 || y0 < 0 || x0 > w - ow || y0 > h - oh) {
-    set_error("%s: the window (%d, %d, %d, %d) leaves the %d x %d input", what, x0, y0, ow, oh, w, h);
-    return VWB200_EARG;
-  }
-  if (rasters_overlap(disparity, w, h, pitch, xyz, ow, oh, xyz_pitch, 12, 24)) { set_error("%s: xyz overlaps the disparity", what); return VWB200_EARG; }
-  return VWB200_OK;
-}
-
-// the raster checks of StereoModel's image form (after the cameras')
-static int model_points_args(const char* what, const float* disparity, int w, int h, ptrdiff_t pitch, const double* xyz, ptrdiff_t xyz_pitch,
-                             const double* error, ptrdiff_t error_pitch) {
-  if (w <= 0 || h <= 0 || pitch < w) { set_error("%s: bad input size %d x %d, pitch %td", what, w, h, pitch); return VWB200_EARG; }
-  if (xyz_pitch < w || error_pitch < w) { set_error("%s: output pitches %td, %td are below the width %d", what, xyz_pitch, error_pitch, w); return VWB200_EARG; }
-  if (rasters_overlap(disparity, w, h, pitch, xyz, w, h, xyz_pitch, 12, 24) || rasters_overlap(disparity, w, h, pitch, error, w, h, error_pitch, 12, 8) ||
-      rasters_overlap(xyz, w, h, xyz_pitch, error, w, h, error_pitch, 24, 8)) {
-    set_error("%s: the disparity, xyz and error rasters overlap", what);
-    return VWB200_EARG;
-  }
-  return VWB200_OK;
-}
-
-int vwb200_universe_radius(const double* in, int w, int h, ptrdiff_t pitch, const double origin[3], double near_radius, double far_radius,
-                           double* out, ptrdiff_t out_pitch, long long* rejected, long long* total, int on_device, void* stream) {
-  const char* what = "UniverseRadius";
-  if (!in || !out || !origin) { set_error("%s: null input, output or origin", what); return VWB200_EARG; }
-  if (w <= 0 || h <= 0 || pitch < w || out_pitch < w) { set_error("%s: bad size %d x %d, pitches %td, %td", what, w, h, pitch, out_pitch); return VWB200_EARG; }
-  if (!(near_radius >= 0 && far_radius >= 0)) { set_error("%s: radii must be >= 0.", what); return VWB200_EARG; }      // StereoView.h:160-163
-  if (!(near_radius <= far_radius)) { set_error("%s: near radius must be <= far radius.", what); return VWB200_EARG; }
-  if (!(out == in && out_pitch == pitch) && rasters_overlap(in, w, h, pitch, out, w, h, out_pitch, 24, 24)) {
-    set_error("%s: out overlaps in (only out == in, with the same pitch, is allowed)", what);
-    return VWB200_EARG;
-  }
-  VWB_TRY(ensure_device());
-  AbiCall c;
-  VWB_TRY(c.open(stream, on_device));
-  const Pt3* din; ptrdiff_t dp;
-  VWB_TRY(c.in((const Pt3*)in, w, h, pitch, on_device, &din, &dp));
-  Pt3* dout; ptrdiff_t dop;
-  VWB_TRY(c.out((Pt3*)out, w, h, out_pitch, on_device, &dout, &dop));
-  unsigned long long* dst;
-  VWB_TRY(tri_stats_open(c, &dst));
-  VWB_TRY(universe_radius_launch((const double*)din, w, h, dp, origin, near_radius, far_radius, (double*)dout, dop, dst, c.st));
-  unsigned long long s[5];
-  VWB_CUDA(cudaMemcpyAsync(s, dst, sizeof s, cudaMemcpyDeviceToHost, c.st));
-  VWB_TRY(c.finish());
-  if (rejected) *rejected = (long long)s[0];
-  if (total) *total = (long long)w * h;
-  return VWB200_OK;
-}
-
-// ---- epipolar rectification (Camera/PinholeModel.cc:679-732, EpipolarUtils.cc:37-76, CameraTransform.h) -----------------------
-static void cross3h(const double* a, const double* b, double* r) {
-  r[0] = a[1] * b[2] - a[2] * b[1];
-  r[1] = a[2] * b[0] - a[0] * b[2];
-  r[2] = a[0] * b[1] - a[1] * b[0];
-}
-
-// camera_pose().rotation_matrix(): Quaternion(R) (Math/Quaternion.h:211-252), branching on the largest of ww, xx, yy, zz, then
-// rotation_matrix() (:314-335)
-static void quaternion_round_trip(const double* R, double* out) {
-  const double d0 = R[0], d1 = R[4], d2 = R[8];
-  const double ww = 1.0 + d0 + d1 + d2, xx = 1.0 + d0 - d1 - d2, yy = 1.0 - d0 + d1 - d2, zz = 1.0 - d0 - d1 + d2;
-  double mx = ww;
-  if (xx > mx) mx = xx;
-  if (yy > mx) mx = yy;
-  if (zz > mx) mx = zz;
-  double q[4];
-  if (ww == mx) {
-    const double w4 = std::sqrt(ww * 4.0);
-    q[0] = w4 / 4; q[1] = (R[7] - R[5]) / w4; q[2] = (R[2] - R[6]) / w4; q[3] = (R[3] - R[1]) / w4;
-  } else if (xx == mx) {
-    const double x4 = std::sqrt(xx * 4.0);
-    q[0] = (R[7] - R[5]) / x4; q[1] = x4 / 4; q[2] = (R[1] + R[3]) / x4; q[3] = (R[2] + R[6]) / x4;
-  } else if (yy == mx) {
-    const double y4 = std::sqrt(yy * 4.0);
-    q[0] = (R[2] - R[6]) / y4; q[1] = (R[1] + R[3]) / y4; q[2] = y4 / 4; q[3] = (R[5] + R[7]) / y4;
-  } else {
-    const double z4 = std::sqrt(zz * 4.0);
-    q[0] = (R[3] - R[1]) / z4; q[1] = (R[2] + R[6]) / z4; q[2] = (R[5] + R[7]) / z4; q[3] = z4 / 4;
-  }
-  const double w = q[0], x = q[1], y = q[2], z = q[3];
-  const double w2 = w * w, x2 = x * x, y2 = y * y, z2 = z * z, wx = w * x, wy = w * y, wz = w * z, xy = x * y, yz = y * z, zx = z * x;
-  out[0] = w2 + x2 - y2 - z2; out[4] = w2 - x2 + y2 - z2; out[8] = w2 - x2 - y2 + z2;
-  out[1] = 2 * (xy - wz); out[2] = 2 * (zx + wy); out[5] = 2 * (yz - wx);
-  out[3] = 2 * (xy + wz); out[6] = 2 * (zx - wy); out[7] = 2 * (yz + wx);
-}
-
-int vwb200_pinhole_epipolar(const vwb200_pinhole* cam0, const vwb200_pinhole* cam1, vwb200_pinhole* epi0, vwb200_pinhole* epi1) {
-  const char* what = "epipolar";
-  if (!epi0 || !epi1) { set_error("%s: null output camera", what); return VWB200_EARG; }
-  VWB_TRY(pinhole_check(what, cam0));
-  VWB_TRY(pinhole_check(what, cam1));
-  TriCam t;
-  VWB_TRY(pinhole_build(what, *cam0, &t));                  // the source cameras must be ones the reference can construct
-  VWB_TRY(pinhole_build(what, *cam1, &t));
-  double rot0[9], rot1[9];
-  quaternion_round_trip(cam0->rotation, rot0);
-  quaternion_round_trip(cam1->rotation, rot1);
-  const double look0[3] = {-1 * rot0[2], -1 * rot0[5], -1 * rot0[8]}, look1[3] = {-1 * rot1[2], -1 * rot1[5], -1 * rot1[8]};
-  double d[3], u[3], mean[3], t1[3], tmp[3], w[3], v[3];
-  for (int i = 0; i < 3; ++i) d[i] = cam1->center[i] - cam0->center[i];
-  const double nd = std::sqrt(dot3h(d, d));
-  for (int i = 0; i < 3; ++i) { u[i] = d[i] / nd; mean[i] = (look0[i] + look1[i]) / 2.0; }
-  cross3h(mean, u, t1);
-  cross3h(u, t1, tmp);
-  const double nt = std::sqrt(dot3h(tmp, tmp));
-  for (int i = 0; i < 3; ++i) w[i] = tmp[i] / nt;
-  cross3h(w, u, v);
-  vwb200_pinhole e{};
-  for (int i = 0; i < 3; ++i) { e.rotation[3 * i] = u[i]; e.rotation[3 * i + 1] = -v[i]; e.rotation[3 * i + 2] = -w[i]; }
-  e.fu = (cam0->fu + cam1->fu) / 2.0; e.fv = (cam0->fv + cam1->fv) / 2.0;
-  e.cu = (cam0->cu + cam1->cu) / 2.0; e.cv = (cam0->cv + cam1->cv) / 2.0;
-  e.pixel_pitch = (cam0->pixel_pitch + cam1->pixel_pitch) / 2.0;
-  e.u_direction[0] = e.v_direction[1] = e.w_direction[2] = 1.0;
-  e.lens = VWB200_LENS_NULL;
-  vwb200_pinhole e1 = e;                                    // the outputs may be the inputs
-  std::memcpy(e.center, cam0->center, sizeof e.center);
-  std::memcpy(e1.center, cam1->center, sizeof e.center);
-  *epi0 = e;
-  *epi1 = e1;
-  return VWB200_OK;
-}
-
-struct MaskF { float v, valid; };                                // PixelMask<float>
-
-// CameraTransform's VW_ASSERT (CameraTransform.h:53, 66): both cameras at one center
-static int same_center(const char* what, const double* a, const double* b) {
-  if (a[0] == b[0] && a[1] == b[1] && a[2] == b[2]) return VWB200_OK;
-  set_error("%s: CameraTransformFunctor: Camera transformation require that the camera center is always the same for both cameras.", what);
-  return VWB200_ELOGIC;
-}
-
-static int projection_error(const char* what, long long x, long long y) {
-  set_error("%s: PinholeModel: Projection into pinhole camera is inaccurate. (first failing pixel (%lld, %lld))", what, x, y);
-  return VWB200_EPROJECT;
-}
-
-// the perimeter index k of compute_transformed_bbox_fast over (x0, y0, x1, y1) as a pixel
-static void perimeter_pixel(const int32_t* r, long long k, long long* x, long long* y) {
-  const long long cw = (long long)r[2] - r[0], ch = (long long)r[3] - r[1];
-  if (k < cw) { *x = r[0] + k; *y = r[1]; }
-  else if (k < 2 * cw) { *x = r[0] + k - cw; *y = r[3] - 1LL; }
-  else if (k < 2 * cw + ch) { *x = r[0]; *y = r[1] + k - 2 * cw; }
-  else { *x = r[2] - 1LL; *y = r[1] + k - 2 * cw - ch; }
-}
-
-static float key_float(unsigned k) {                           // kfloat on the host
-  const unsigned u = (k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k;
-  float f;
-  std::memcpy(&f, &u, sizeof f);
-  return f;
-}
-static unsigned float_key(float f) {
-  unsigned u;
-  std::memcpy(&u, &f, sizeof u);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-
-// both cameras' compute_transformed_bbox_fast through CameraTransform(cam, epi)::forward: bbox[cam] = {min x, min y, max x, max y}
-static int epipolar_bboxes(AbiCall& c, const TriCam* cam, const TriCam* epi, const int32_t* const* roi, float (*bbox)[4]) {
-  unsigned* keys;
-  unsigned long long* fail;
-  VWB_TRY(c.ar.alloc(&keys, 8));
-  VWB_TRY(c.ar.alloc(&fail, 4));
-  const float big = (float)(INT32_MAX - 1);                    // BBox2f's initial bounds (Math/BBox.tcc:38-45)
-  const unsigned init[8] = {float_key(big), float_key(big), float_key(-big), float_key(-big),
-                            float_key(big), float_key(big), float_key(-big), float_key(-big)};
-  const unsigned long long finit[4] = {0, ULLONG_MAX, 0, ULLONG_MAX};
-  VWB_CUDA(cudaMemcpyAsync(keys, init, sizeof init, cudaMemcpyHostToDevice, c.st));
-  VWB_CUDA(cudaMemcpyAsync(fail, finit, sizeof finit, cudaMemcpyHostToDevice, c.st));
-  for (int i = 0; i < 2; ++i)
-    VWB_TRY(camera_bbox_launch(cam[i], epi[i], roi[i][0], roi[i][1], roi[i][2], roi[i][3], keys + 4 * i, fail + 2 * i, c.st));
-  unsigned k[8];
-  unsigned long long f[4];
-  VWB_CUDA(cudaMemcpyAsync(k, keys, sizeof k, cudaMemcpyDeviceToHost, c.st));
-  VWB_CUDA(cudaMemcpyAsync(f, fail, sizeof f, cudaMemcpyDeviceToHost, c.st));
-  VWB_CUDA(cudaStreamSynchronize(c.st));
-  for (int i = 0; i < 2; ++i)
-    if (f[2 * i]) {                                            // the reference throws at the first failing point of the first camera
-      long long x, y;
-      perimeter_pixel(roi[i], (long long)f[2 * i + 1], &x, &y);
-      return projection_error("resize_epipolar_cameras_to_fit", x, y);
-    }
-  for (int i = 0; i < 8; ++i) bbox[i / 4][i % 4] = key_float(k[i]);
-  return VWB200_OK;
-}
-
-static int roi_check(const char* what, const int32_t* r) {
-  if (!r) { set_error("%s: null ROI", what); return VWB200_EARG; }
-  if (r[2] < r[0] || r[3] < r[1]) { set_error("%s: bad ROI (%d, %d, %d, %d)", what, r[0], r[1], r[2], r[3]); return VWB200_EARG; }
-  return VWB200_OK;
-}
-
-int vwb200_resize_epipolar_cameras_to_fit(const vwb200_pinhole* cam1, const vwb200_pinhole* cam2, vwb200_pinhole* epi1, vwb200_pinhole* epi2,
-                                          const int32_t roi1[4], const int32_t roi2[4], int32_t size1[2], int32_t size2[2], void* stream) {
-  const char* what = "resize_epipolar_cameras_to_fit";
-  if (!size1 || !size2) { set_error("%s: null output size", what); return VWB200_EARG; }
-  VWB_TRY(pinhole_check(what, cam1));
-  VWB_TRY(pinhole_check(what, cam2));
-  VWB_TRY(pinhole_check(what, epi1));
-  VWB_TRY(pinhole_check(what, epi2));
-  VWB_TRY(roi_check(what, roi1));
-  VWB_TRY(roi_check(what, roi2));
-  TriCam cam[2], epi[2];
-  VWB_TRY(pinhole_build(what, *cam1, &cam[0]));
-  VWB_TRY(pinhole_build(what, *cam2, &cam[1]));
-  VWB_TRY(pinhole_build(what, *epi1, &epi[0]));
-  VWB_TRY(pinhole_build(what, *epi2, &epi[1]));
-  VWB_TRY(same_center(what, cam[0].c, epi[0].c));
-  VWB_TRY(same_center(what, cam[1].c, epi[1].c));
-  VWB_TRY(ensure_device());
-  AbiCall c;
-  VWB_TRY(c.open(stream, 0));
-  const int32_t* roi[2] = {roi1, roi2};
-  float bb[2][4];
-  VWB_TRY(epipolar_bboxes(c, cam, epi, roi, bb));
-  // shift both principal points by the leftmost / uppermost corner (in CCD units), from epi1's offset (EpipolarUtils.cc:52-65)
-  const double min_col = std::min(bb[0][0], bb[1][0]), min_row = std::min(bb[0][1], bb[1][1]);
-  const double cu = epi1->cu - min_col * epi1->pixel_pitch, cv = epi1->cv - min_row * epi1->pixel_pitch;
-  vwb200_pinhole e1 = *epi1, e2 = *epi2;
-  e1.cu = e2.cu = cu;
-  e1.cv = e2.cv = cv;
-  VWB_TRY(pinhole_build(what, e1, &epi[0]));
-  VWB_TRY(pinhole_build(what, e2, &epi[1]));
-  VWB_TRY(epipolar_bboxes(c, cam, epi, roi, bb));
-  VWB_TRY(c.finish());
-  *epi1 = e1;
-  *epi2 = e2;
-  size1[0] = (int32_t)bb[0][2]; size1[1] = (int32_t)bb[0][3];    // Vector2i(bbox.max()): truncation toward zero
-  size2[0] = (int32_t)bb[1][2]; size2[1] = (int32_t)bb[1][3];
-  return VWB200_OK;
-}
-
-// the raster, pixel type, interpolation and edge checks of camera_transform (after the cameras'): VWB200_EARG, then
-// VWB200_ENOIMPL for the combinations without a device form
-static int camera_transform_args(const char* what, int pixel_type, int interp, int edge, const float* edge_value, const void* in, int w, int h,
-                                 ptrdiff_t pitch, int x0, int y0, const void* out, int ow, int oh, ptrdiff_t opitch) {
-  if (pixel_type != VWB200_PIXEL_GRAY_F32 && pixel_type != VWB200_PIXEL_MASK_F32) { set_error("%s: unknown pixel type %d", what, pixel_type); return VWB200_EARG; }
-  if (interp != VWB200_INTERP_BILINEAR && interp != VWB200_INTERP_BICUBIC && interp != VWB200_INTERP_NEAREST) {
-    set_error("%s: unknown interpolation %d", what, interp);
-    return VWB200_EARG;
-  }
-  if (edge != VWB200_EDGE_ZERO && edge != VWB200_EDGE_CONSTANT && edge != VWB200_EDGE_VALUE) { set_error("%s: unknown edge extension %d", what, edge); return VWB200_EARG; }
-  if (w <= 0 || h <= 0 || pitch < w) { set_error("%s: bad image size %d x %d, pitch %td", what, w, h, pitch); return VWB200_EARG; }
-  if (ow <= 0 || oh <= 0 || opitch < ow) { set_error("%s: bad output size %d x %d, pitch %td", what, ow, oh, opitch); return VWB200_EARG; }
-  if ((long long)x0 + ow - 1 > INT_MAX || (long long)y0 + oh - 1 > INT_MAX) {
-    set_error("%s: the window (%d, %d, %d, %d) leaves the int32 pixel coordinates", what, x0, y0, ow, oh);
-    return VWB200_EARG;
-  }
-  const bool masked = pixel_type == VWB200_PIXEL_MASK_F32;
-  const size_t px = masked ? 8 : 4;
-  if (rasters_overlap(in, w, h, pitch, out, ow, oh, opitch, px, px)) { set_error("%s: out overlaps the image", what); return VWB200_EARG; }
-  if (edge == VWB200_EDGE_VALUE && !edge_value) { set_error("%s: ValueEdgeExtension needs an edge value", what); return VWB200_EARG; }
-  if ((masked && interp != VWB200_INTERP_BILINEAR) || (!masked && edge == VWB200_EDGE_VALUE)) {
-    set_error("%s: %s has no device form (PixelMask<float> takes bilinear interpolation, ValueEdgeExtension PixelMask<float> pixels)", what,
-              masked ? "this interpolation of PixelMask<float> pixels" : "ValueEdgeExtension of float pixels");
-    return VWB200_ENOIMPL;
-  }
-  return VWB200_OK;
-}
-
-// camera_transform's image and window, staged: float pixels, or {value, valid} pairs staged as such
-static int camera_transform_stage(AbiCall& c, bool masked, const void* in, int w, int h, ptrdiff_t pitch, void* out, int ow, int oh, ptrdiff_t opitch,
-                                  int on_device, const float** din, ptrdiff_t* dp, float** dout, ptrdiff_t* dop) {
-  if (masked) {
-    const MaskF* mi; MaskF* mo;
-    VWB_TRY(c.in((const MaskF*)in, w, h, pitch, on_device, &mi, dp));
-    VWB_TRY(c.out((MaskF*)out, ow, oh, opitch, on_device, &mo, dop));
-    *din = (const float*)mi; *dout = (float*)mo;
-    return VWB200_OK;
-  }
-  VWB_TRY(c.in((const float*)in, w, h, pitch, on_device, din, dp));
-  return c.out((float*)out, ow, oh, opitch, on_device, dout, dop);
-}
-
 // ---- the view -------------------------------------------------------------------------------------
-// ---- CAHV / CAHVOR cameras (Camera/CAHVModel.cc, CAHVORModel.cc, CameraTransform.h, StereoModel.cc:121-122) ---------------------
-// The host restatement of the camera math (linearize_camera calls pixel_to_vector); cahv.cuh is the device one.  x86-64 host
-// code has no FMA to contract into, so each operation rounds as the reference's does.
-static void scale3h(double s, const double* a, double* r) { for (int i = 0; i < 3; ++i) r[i] = s * a[i]; }
-static void normalize3h(const double* a, double* r) {          // Math/Vector.h:1694: each component / norm_2
-  const double n = std::sqrt(dot3h(a, a));
-  for (int i = 0; i < 3; ++i) r[i] = a[i] / n;
-}
-// dot_prod(cross_prod(V, H), A) < 0: a left-handed camera, whose rays pixel_to_vector negates
-static bool cahv_left_handed(const vwb200_cahv& c) {
-  double t[3];
-  cross3h(c.V, c.H, t);
-  return dot3h(t, c.A) < 0.0;
-}
-
-static int cahv_check(const char* what, const vwb200_cahv* c) {
-  if (!c) { set_error("%s: null camera", what); return VWB200_EARG; }
-  if (c->model != VWB200_CAMERA_CAHV && c->model != VWB200_CAMERA_CAHVOR) { set_error("%s: unknown camera model %d", what, c->model); return VWB200_EARG; }
-  return VWB200_OK;
-}
-
-// CAHVORModel::pixel_to_vector(pix), the overload without partial derivatives (CAHVORModel.cc:297-348)
-static void cahvor_pixel_to_vector(const vwb200_cahv& c, double x, double y, double* out) {
-  double f[3], g[3], t[3], rr[3], lambda[3];
-  for (int i = 0; i < 3; ++i) { f[i] = c.V[i] - y * c.A[i]; g[i] = c.H[i] - x * c.A[i]; }
-  cross3h(f, g, t);
-  normalize3h(t, rr);
-  if (cahv_left_handed(c)) scale3h(-1.0, rr, rr);
-  const double omega = dot3h(rr, c.O);
-  for (int i = 0; i < 3; ++i) lambda[i] = rr[i] - omega * c.O[i];
-  const double tau = dot3h(lambda, lambda) / (omega * omega);
-  const double k1 = 1 + c.R[0], k3 = c.R[1] * tau, k5 = c.R[2] * tau * tau;
-  double u = 1.0 - (c.R[0] + k3 + k5);
-  for (int i = 0;; i++) {
-    if (i >= 20) break;                                          // VW_CAHVOR_MAXITER
-    const double u_2 = u * u;
-    const double poly = ((k5 * u_2 + k3) * u_2 + k1) * u - 1;
-    const double deriv = (5 * k5 * u_2 + 3 * k3) * u_2 + k1;
-    if (deriv <= 0) break;
-    const double du = poly / deriv;
-    u -= du;
-    if (std::fabs(du) < 1.0e-6) break;                           // VW_CAHVOR_CONV
-  }
-  for (int i = 0; i < 3; ++i) t[i] = rr[i] - (1 - u) * lambda[i];
-  normalize3h(t, out);
-}
-
-int vwb200_cahv_epipolar(const vwb200_cahv* cam0, const vwb200_cahv* cam1, vwb200_cahv* epi0, vwb200_cahv* epi1) {
-  const char* what = "epipolar";
-  if (!epi0 || !epi1) { set_error("%s: null output camera", what); return VWB200_EARG; }
-  VWB_TRY(cahv_check(what, cam0));
-  VWB_TRY(cahv_check(what, cam1));
-  if (cam0->model != VWB200_CAMERA_CAHV || cam1->model != VWB200_CAMERA_CAHV) {
-    set_error("%s: epipolar() takes CAHV cameras (linearize_camera takes a CAHVOR camera to one)", what);
-    return VWB200_EARG;
-  }
-  const vwb200_cahv& s0 = *cam0;
-  const vwb200_cahv& s1 = *cam1;
-  double t[3];
-  const double hc = dot3h(s0.H, s0.A) / 2.0 + dot3h(s1.H, s1.A) / 2.0;
-  const double vc = dot3h(s0.V, s0.A) / 2.0 + dot3h(s1.V, s1.A) / 2.0;
-  cross3h(s0.A, s0.H, t);
-  double hs = std::sqrt(dot3h(t, t)) / 2.0;
-  cross3h(s1.A, s1.H, t);
-  hs = hs + std::sqrt(dot3h(t, t)) / 2.0;
-  cross3h(s0.A, s0.V, t);
-  double vs = std::sqrt(dot3h(t, t)) / 2.0;
-  cross3h(s1.A, s1.V, t);
-  vs = vs + std::sqrt(dot3h(t, t)) / 2.0;
-  double app[3], dc[3], f[3], hp[3], g[3], a[3], vp[3];
-  for (int i = 0; i < 3; ++i) { app[i] = s0.A[i] + s1.A[i]; dc[i] = s1.C[i] - s0.C[i]; }
-  cross3h(app, dc, t);
-  cross3h(t, app, f);
-  const double nf = std::sqrt(dot3h(f, f));
-  if (dot3h(f, s0.H) > 0)
-    for (int i = 0; i < 3; ++i) hp[i] = f[i] * hs / nf;
-  else
-    for (int i = 0; i < 3; ++i) hp[i] = -f[i] * hs / nf;
-  for (int i = 0; i < 3; ++i) app[i] *= 0.5;
-  const double dh = dot3h(app, hp);
-  for (int i = 0; i < 3; ++i) { g[i] = hp[i] * dh / (hs * hs); t[i] = app[i] - g[i]; }
-  normalize3h(t, a);
-  cross3h(a, hp, t);
-  for (int i = 0; i < 3; ++i) vp[i] = t[i] * vs / hs;
-  vwb200_cahv e{};
-  e.model = VWB200_CAMERA_CAHV;
-  for (int i = 0; i < 3; ++i) { e.A[i] = a[i]; e.H[i] = hp[i] + hc * a[i]; e.V[i] = vp[i] + vc * a[i]; }
-  vwb200_cahv e1 = e;                                            // the outputs may be the inputs
-  std::memcpy(e.C, s0.C, sizeof e.C);
-  std::memcpy(e1.C, s1.C, sizeof e1.C);
-  *epi0 = e;
-  *epi1 = e1;
-  return VWB200_OK;
-}
-
-int vwb200_linearize_camera(const vwb200_cahv* cam, const int32_t cahvor_size[2], const int32_t cahv_size[2], vwb200_cahv* out) {
-  const char* what = "linearize_camera";
-  if (!cahvor_size || !cahv_size || !out) { set_error("%s: null size or output camera", what); return VWB200_EARG; }
-  VWB_TRY(cahv_check(what, cam));
-  if (cam->model != VWB200_CAMERA_CAHVOR) { set_error("%s: linearize_camera() takes a CAHVOR camera", what); return VWB200_EARG; }
-  const vwb200_cahv c = *cam;                                    // out may be cam
-  const int ix = cahvor_size[0], iy = cahvor_size[1];
-  // the landmarks around the perimeter; vpts[4] divides in int where vpts[1] divides in double, as the reference does
-  const double hpts[6][2] = {{0, 0}, {0, (iy - 1) / 2.0}, {0, (double)(iy - 1)}, {(double)(ix - 1), 0}, {(double)(ix - 1), (iy - 1) / 2.0},
-                             {ix - 1.0, iy - 1.0}};
-  const double vpts[6][2] = {{0, 0}, {(ix - 1) / 2.0, 0}, {(double)(ix - 1), 0}, {0, (double)(iy - 1)}, {(double)((ix - 1) / 2), (double)(iy - 1)},
-                             {ix - 1.0, iy - 1.0}};
-  double A[3] = {0.0, 0.0, 0.0}, r[3];
-  for (int k = 0; k < 6; ++k) { cahvor_pixel_to_vector(c, vpts[k][0], vpts[k][1], r); for (int i = 0; i < 3; ++i) A[i] += r[i]; }
-  for (int k = 0; k < 6; ++k) { cahvor_pixel_to_vector(c, hpts[k][0], hpts[k][1], r); for (int i = 0; i < 3; ++i) A[i] += r[i]; }
-  normalize3h(A, A);
-  double dn[3], rt[3], t[3];
-  cross3h(c.A, c.H, dn);
-  cross3h(dn, c.A, t);
-  normalize3h(t, rt);
-  normalize3h(dn, dn);
-  cross3h(dn, A, rt);
-  cross3h(A, rt, t);
-  normalize3h(t, dn);
-  normalize3h(rt, rt);
-  double hmin = 1, hmax = -1, vmin = 1, vmax = -1;
-  for (int k = 0; k < 6; ++k) {
-    double u3[3], w3[3];
-    cahvor_pixel_to_vector(c, hpts[k][0], hpts[k][1], u3);
-    const double d = dot3h(dn, u3);
-    for (int i = 0; i < 3; ++i) t[i] = u3[i] - d * dn[i];
-    normalize3h(t, w3);
-    cross3h(A, w3, t);
-    const double sn = std::sqrt(dot3h(t, t));
-    if (hmin > sn) hmin = sn;
-    if (hmax < sn) hmax = sn;
-  }
-  for (int k = 0; k < 6; ++k) {
-    double u3[3], w3[3];
-    cahvor_pixel_to_vector(c, vpts[k][0], vpts[k][1], u3);
-    const double d = dot3h(rt, u3);
-    for (int i = 0; i < 3; ++i) t[i] = u3[i] - d * rt[i];
-    normalize3h(t, w3);
-    cross3h(A, w3, t);
-    const double sn = std::sqrt(dot3h(t, t));
-    if (vmin > sn) vmin = sn;
-    if (vmax < sn) vmax = sn;
-  }
-  // minfov: the smaller field of view
-  const double ic[2] = {((double)cahv_size[0] - 1.0) / 2.0, ((double)cahv_size[1] - 1.0) / 2.0};
-  const double ic2[2] = {ic[0] * ic[0], ic[1] * ic[1]};
-  const double sf[2] = {std::sqrt(ic2[0] / (hmin * hmin) - ic2[0]), std::sqrt(ic2[1] / (vmin * vmin) - ic2[1])};
-  vwb200_cahv o{};
-  o.model = VWB200_CAMERA_CAHV;
-  for (int i = 0; i < 3; ++i) {
-    o.C[i] = c.C[i];
-    o.A[i] = A[i];
-    o.H[i] = sf[0] * rt[i] + ic[0] * A[i];
-    o.V[i] = sf[1] * dn[i] + ic[1] * A[i];
-  }
-  *out = o;
-  return VWB200_OK;
-}
-
-int vwb200_pinhole_to_cahv(const vwb200_pinhole* pin, vwb200_cahv* out) {
-  const char* what = "CAHVModel = PinholeModel";
-  if (!out) { set_error("%s: null output camera", what); return VWB200_EARG; }
-  VWB_TRY(pinhole_check(what, pin));
-  if (pin->lens != VWB200_LENS_NULL) { set_error("%s: the pinhole has a lens distortion, which a CAHV camera cannot carry", what); return VWB200_EARG; }
-  TriCam t;
-  VWB_TRY(pinhole_build(what, *pin, &t));                        // a camera the reference can construct
-  const double pitch = pin->pixel_pitch;
-  if (pitch == 0) { set_error("%s: CAHVModel::operator=() input pinhole model has zero pitch!", what); return VWB200_EARG; }
-  const double fH = pin->fu / pitch, fV = pin->fv / pitch, cH = pin->cu / pitch, cV = pin->cv / pitch;
-  double Hv[3], Vv[3], A[3];
-  for (int i = 0; i < 3; ++i) {                                  // R * u, R * v, R * w: row i of R . the vector, from 0.0
-    Hv[i] = dot3h(pin->rotation + 3 * i, pin->u_direction);
-    Vv[i] = dot3h(pin->rotation + 3 * i, pin->v_direction);
-    A[i] = dot3h(pin->rotation + 3 * i, pin->w_direction);
-  }
-  vwb200_cahv o{};
-  o.model = VWB200_CAMERA_CAHV;
-  for (int i = 0; i < 3; ++i) {
-    o.C[i] = pin->center[i];
-    o.A[i] = A[i];
-    o.H[i] = fH * Hv[i] + cH * A[i];
-    o.V[i] = fV * Vv[i] + cV * A[i];
-  }
-  *out = o;
-  return VWB200_OK;
-}
-
-// ---- stereo_triangulate, StereoModel and camera_transform through either camera family -----------------------------------
-// What these calls need to know of a family: its C ABI and device cameras, the argument check, build (VWB200_ELOGIC / EMATH for
-// a pinhole camera the reference cannot construct), the center, the statistic that receives the Newton iterations, and which
-// camera_transform destinations have a device form.  The family bodies are templates, so they sit in an extern "C++" block.
-extern "C++" {
-struct PinholeFamily {
-  using Abi = vwb200_pinhole;
-  using Dev = TriCam;
-  static constexpr auto check = pinhole_check;
-  static constexpr auto build = pinhole_build;
-  static const double* center(const TriCam& c) { return c.c; }
-  static constexpr long long vwb200_triangulation_stats::*iterations = &vwb200_triangulation_stats::tsai_iterations;
-  static int transform_dst(const char*, const vwb200_pinhole&) { return VWB200_OK; }
-};
-struct CahvFamily {
-  using Abi = vwb200_cahv;
-  using Dev = CahvCam;
-  static constexpr auto check = cahv_check;
-  static int build(const char*, const vwb200_cahv& c, CahvCam* d) {
-    std::memcpy(d->C, c.C, sizeof d->C); std::memcpy(d->A, c.A, sizeof d->A); std::memcpy(d->H, c.H, sizeof d->H);
-    std::memcpy(d->V, c.V, sizeof d->V); std::memcpy(d->O, c.O, sizeof d->O); std::memcpy(d->R, c.R, sizeof d->R);
-    d->cahvor = c.model == VWB200_CAMERA_CAHVOR;
-    d->flip = cahv_left_handed(c);
-    return VWB200_OK;
-  }
-  static const double* center(const CahvCam& c) { return c.C; }
-  static constexpr long long vwb200_triangulation_stats::*iterations = &vwb200_triangulation_stats::cahvor_iterations;
-  // K8 compiles the destination's ray without the CAHVOR Newton loop
-  static int transform_dst(const char* what, const vwb200_cahv& c) {
-    if (c.model == VWB200_CAMERA_CAHV) return VWB200_OK;
-    set_error("%s: the destination camera must be CAHV (a CAHVOR one has no device form)", what);
-    return VWB200_ENOIMPL;
-  }
-};
-
-template <class F>
-static int stereo_triangulate_family(int pixel_type, const void* disparity, int w, int h, ptrdiff_t pitch, int x0, int y0, int ow, int oh,
-                                     const typename F::Abi* cam1, const typename F::Abi* cam2, double angle_tol, double* xyz,
-                                     ptrdiff_t xyz_pitch, int on_device, void* stream) {
-  t_tri_stats = vwb200_triangulation_stats{};
-  const char* what = "stereo_triangulate";
-  if (!disparity || !xyz) { set_error("%s: null disparity or output", what); return VWB200_EARG; }
-  if (pixel_type != VWB200_DISP_I32 && pixel_type != VWB200_DISP_F32) { set_error("%s: unknown pixel type %d", what, pixel_type); return VWB200_EARG; }
-  VWB_TRY(F::check(what, cam1));
-  VWB_TRY(F::check(what, cam2));
-  VWB_TRY(triangulate_args(what, disparity, w, h, pitch, x0, y0, ow, oh, xyz, xyz_pitch));
-  typename F::Dev c0, c1;
-  VWB_TRY(F::build(what, *cam1, &c0));
-  VWB_TRY(F::build(what, *cam2, &c1));
-  const double tol = angle_tol > 0 ? angle_tol : 1e-4;            // are_nearly_parallel's (StereoModel.cc:81-83)
-  VWB_TRY(ensure_device());
-  AbiCall c;
-  VWB_TRY(c.open(stream, on_device));
-  Pt3* dxyz; ptrdiff_t dxp;
-  VWB_TRY(c.out((Pt3*)xyz, ow, oh, xyz_pitch, on_device, &dxyz, &dxp));
-  unsigned long long* dst;
-  VWB_TRY(tri_stats_open(c, &dst));
-  // only the window is read: stage that alone
-  if (pixel_type == VWB200_DISP_I32) {
-    const vwb200_dispi* din; ptrdiff_t dp;
-    VWB_TRY(c.in((const vwb200_dispi*)disparity + (ptrdiff_t)y0 * pitch + x0, ow, oh, pitch, on_device, &din, &dp));
-    VWB_TRY(stereo_triangulate_launch(din, dp, x0, y0, ow, oh, c0, c1, tol, (double*)dxyz, dxp, dst, c.st));
-  } else {
-    const DispF* din; ptrdiff_t dp;
-    VWB_TRY(c.in((const DispF*)disparity + (ptrdiff_t)y0 * pitch + x0, ow, oh, pitch, on_device, &din, &dp));
-    VWB_TRY(stereo_triangulate_launch(din, dp, x0, y0, ow, oh, c0, c1, tol, (double*)dxyz, dxp, dst, c.st));
-  }
-  unsigned long long s[5];
-  VWB_CUDA(cudaMemcpyAsync(s, dst, sizeof s, cudaMemcpyDeviceToHost, c.st));
-  VWB_TRY(c.finish());
-  t_tri_stats.*F::iterations = (long long)s[4];
-  return VWB200_OK;
-}
-
-template <class F>
-static int stereo_model_points_family(const float* disparity, int w, int h, ptrdiff_t pitch, const typename F::Abi* cam1,
-                                      const typename F::Abi* cam2, double angle_tol, double* xyz, ptrdiff_t xyz_pitch, double* error,
-                                      ptrdiff_t error_pitch, int on_device, void* stream) {
-  t_tri_stats = vwb200_triangulation_stats{};
-  const char* what = "StereoModel";
-  if (!disparity || !xyz || !error) { set_error("%s: null disparity or output", what); return VWB200_EARG; }
-  VWB_TRY(F::check(what, cam1));
-  VWB_TRY(F::check(what, cam2));
-  VWB_TRY(model_points_args(what, disparity, w, h, pitch, xyz, xyz_pitch, error, error_pitch));
-  typename F::Dev c0, c1;
-  VWB_TRY(F::build(what, *cam1, &c0));
-  VWB_TRY(F::build(what, *cam2, &c1));
-  const double tol = angle_tol > 0 ? angle_tol : 1e-4;
-  VWB_TRY(ensure_device());
-  AbiCall c;
-  VWB_TRY(c.open(stream, on_device));
-  const DispF* din; ptrdiff_t dp;
-  VWB_TRY(c.in((const DispF*)disparity, w, h, pitch, on_device, &din, &dp));
-  Pt3* dxyz; ptrdiff_t dxp;
-  VWB_TRY(c.out((Pt3*)xyz, w, h, xyz_pitch, on_device, &dxyz, &dxp));
-  double* derr; ptrdiff_t dep;
-  VWB_TRY(c.out(error, w, h, error_pitch, on_device, &derr, &dep));
-  unsigned long long* dst;
-  VWB_TRY(tri_stats_open(c, &dst));
-  VWB_TRY(stereo_model_launch(din, w, h, dp, c0, c1, tol, (double*)dxyz, dxp, derr, dep, dst, c.st));
-  unsigned long long s[5];
-  VWB_CUDA(cudaMemcpyAsync(s, dst, sizeof s, cudaMemcpyDeviceToHost, c.st));
-  VWB_TRY(c.finish());
-  double sum, mx;
-  std::memcpy(&sum, &s[0], sizeof sum);
-  std::memcpy(&mx, &s[1], sizeof mx);
-  t_tri_stats = vwb200_triangulation_stats{(long long)s[2], (long long)s[3], mx, sum, 0, 0};
-  t_tri_stats.*F::iterations = (long long)s[4];
-  return VWB200_OK;
-}
-
-template <class F>
-static int camera_transform_family(const typename F::Abi* src, const typename F::Abi* dst, int pixel_type, int interp, int edge,
-                                   const float* edge_value, const void* in, int w, int h, ptrdiff_t pitch, int x0, int y0, void* out, int ow,
-                                   int oh, ptrdiff_t opitch, int on_device, void* stream) {
-  const char* what = "camera_transform";
-  if (!in || !out) { set_error("%s: null input or output", what); return VWB200_EARG; }
-  VWB_TRY(F::check(what, src));
-  VWB_TRY(F::check(what, dst));
-  VWB_TRY(camera_transform_args(what, pixel_type, interp, edge, edge_value, in, w, h, pitch, x0, y0, out, ow, oh, opitch));
-  VWB_TRY(F::transform_dst(what, *dst));
-  const bool masked = pixel_type == VWB200_PIXEL_MASK_F32;
-  const float ev[2] = {edge_value ? edge_value[0] : 0.0f, edge_value ? edge_value[1] : 0.0f};
-  typename F::Dev s, d;
-  VWB_TRY(F::build(what, *src, &s));
-  VWB_TRY(F::build(what, *dst, &d));
-  VWB_TRY(same_center(what, F::center(s), F::center(d)));
-  VWB_TRY(ensure_device());
-  AbiCall c;
-  VWB_TRY(c.open(stream, on_device));
-  const float* din; ptrdiff_t dp;
-  float* dout; ptrdiff_t dop;
-  VWB_TRY(camera_transform_stage(c, masked, in, w, h, pitch, out, ow, oh, opitch, on_device, &din, &dp, &dout, &dop));
-  unsigned long long* fail;
-  VWB_TRY(c.ar.alloc(&fail, 2));
-  const unsigned long long finit[2] = {0, ULLONG_MAX};
-  VWB_CUDA(cudaMemcpyAsync(fail, finit, sizeof finit, cudaMemcpyHostToDevice, c.st));
-  VWB_TRY(camera_warp_launch(masked, interp, edge, ev, s, d, din, w, h, dp, x0, y0, dout, ow, oh, dop, fail, c.st));
-  unsigned long long f[2];
-  VWB_CUDA(cudaMemcpyAsync(f, fail, sizeof f, cudaMemcpyDeviceToHost, c.st));
-  VWB_TRY(c.finish());
-  if (f[0]) return projection_error(what, x0 + (long long)(f[1] % (unsigned long long)ow), y0 + (long long)(f[1] / (unsigned long long)ow));
-  return VWB200_OK;
-}
-}  // extern "C++"
-
-int vwb200_stereo_triangulate(int pixel_type, const void* disparity, int w, int h, ptrdiff_t pitch, int x0, int y0, int ow, int oh,
-                              const vwb200_pinhole* cam1, const vwb200_pinhole* cam2, double angle_tol, double* xyz, ptrdiff_t xyz_pitch,
-                              int on_device, void* stream) {
-  return stereo_triangulate_family<PinholeFamily>(pixel_type, disparity, w, h, pitch, x0, y0, ow, oh, cam1, cam2, angle_tol, xyz, xyz_pitch,
-                                                  on_device, stream);
-}
-
-int vwb200_cahv_stereo_triangulate(int pixel_type, const void* disparity, int w, int h, ptrdiff_t pitch, int x0, int y0, int ow, int oh,
-                                   const vwb200_cahv* cam1, const vwb200_cahv* cam2, double angle_tol, double* xyz, ptrdiff_t xyz_pitch,
-                                   int on_device, void* stream) {
-  return stereo_triangulate_family<CahvFamily>(pixel_type, disparity, w, h, pitch, x0, y0, ow, oh, cam1, cam2, angle_tol, xyz, xyz_pitch,
-                                               on_device, stream);
-}
-
-int vwb200_stereo_model_points(const float* disparity, int w, int h, ptrdiff_t pitch, const vwb200_pinhole* cam1,
-                               const vwb200_pinhole* cam2, double angle_tol, double* xyz, ptrdiff_t xyz_pitch, double* error,
-                               ptrdiff_t error_pitch, int on_device, void* stream) {
-  return stereo_model_points_family<PinholeFamily>(disparity, w, h, pitch, cam1, cam2, angle_tol, xyz, xyz_pitch, error, error_pitch,
-                                                   on_device, stream);
-}
-
-int vwb200_cahv_stereo_model_points(const float* disparity, int w, int h, ptrdiff_t pitch, const vwb200_cahv* cam1, const vwb200_cahv* cam2,
-                                    double angle_tol, double* xyz, ptrdiff_t xyz_pitch, double* error, ptrdiff_t error_pitch, int on_device,
-                                    void* stream) {
-  return stereo_model_points_family<CahvFamily>(disparity, w, h, pitch, cam1, cam2, angle_tol, xyz, xyz_pitch, error, error_pitch, on_device,
-                                                stream);
-}
-
-int vwb200_camera_transform(const vwb200_pinhole* src, const vwb200_pinhole* dst, int pixel_type, int interp, int edge, const float edge_value[2],
-                            const void* in, int w, int h, ptrdiff_t pitch, int x0, int y0, void* out, int ow, int oh, ptrdiff_t opitch,
-                            int on_device, void* stream) {
-  return camera_transform_family<PinholeFamily>(src, dst, pixel_type, interp, edge, edge_value, in, w, h, pitch, x0, y0, out, ow, oh, opitch,
-                                                on_device, stream);
-}
-
-int vwb200_cahv_camera_transform(const vwb200_cahv* src, const vwb200_cahv* dst, int pixel_type, int interp, int edge, const float edge_value[2],
-                                 const void* in, int w, int h, ptrdiff_t pitch, int x0, int y0, void* out, int ow, int oh, ptrdiff_t opitch,
-                                 int on_device, void* stream) {
-  return camera_transform_family<CahvFamily>(src, dst, pixel_type, interp, edge, edge_value, in, w, h, pitch, x0, y0, out, ow, oh, opitch,
-                                             on_device, stream);
-}
-
 int vwb200_corr_create(const vwb200_corr_params* p, vwb200_corr** out) {
   if (!p || !out) { set_error("corr_create: null pointer"); return VWB200_EARG; }
   const double w = (double)p->search_x1 - p->search_x0, h = (double)p->search_y1 - p->search_y0;

@@ -4,8 +4,11 @@
 // and the pixel_to_vector round-trip check.  The camera is a TriCam the host builds once per call.  Every product, sum,
 // quotient and square root is an explicitly rounded intrinsic in the reference's order -- dot products and norms are sums from
 // 0.0 (Math/Vector.h:1593-1604, 1717-1726) -- so nothing is contracted into an FMA and the doubles are the reference's bit for bit.
+// The primitives and vector helpers are also the host's (cameras.cu builds and rectifies cameras with them): there each is the
+// plain operator, which build.py's -ffp-contract=off keeps the host compiler from contracting.
 #pragma once
 #include <cfloat>
+#include <cmath>
 
 #include "common.cuh"
 
@@ -14,18 +17,28 @@ namespace {
 
 struct V3 { double x, y, z; };
 
-__device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a, b); }
-__device__ __forceinline__ double dsub(double a, double b) { return __dsub_rn(a, b); }
-__device__ __forceinline__ double dmul(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ double ddiv(double a, double b) { return __ddiv_rn(a, b); }
+#ifdef __CUDA_ARCH__
+__host__ __device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a, b); }
+__host__ __device__ __forceinline__ double dsub(double a, double b) { return __dsub_rn(a, b); }
+__host__ __device__ __forceinline__ double dmul(double a, double b) { return __dmul_rn(a, b); }
+__host__ __device__ __forceinline__ double ddiv(double a, double b) { return __ddiv_rn(a, b); }
+__host__ __device__ __forceinline__ double dsqrt(double a) { return __dsqrt_rn(a); }
+#else
+__host__ __device__ __forceinline__ double dadd(double a, double b) { return a + b; }
+__host__ __device__ __forceinline__ double dsub(double a, double b) { return a - b; }
+__host__ __device__ __forceinline__ double dmul(double a, double b) { return a * b; }
+__host__ __device__ __forceinline__ double ddiv(double a, double b) { return a / b; }
+__host__ __device__ __forceinline__ double dsqrt(double a) { return std::sqrt(a); }
+#endif
 
-__device__ __forceinline__ V3 sub3(V3 a, V3 b) { return V3{dsub(a.x, b.x), dsub(a.y, b.y), dsub(a.z, b.z)}; }
+__host__ __device__ __forceinline__ V3 ld3(const double* p) { return V3{p[0], p[1], p[2]}; }
+__host__ __device__ __forceinline__ V3 sub3(V3 a, V3 b) { return V3{dsub(a.x, b.x), dsub(a.y, b.y), dsub(a.z, b.z)}; }
 // dot_prod: a sum from 0.0 (so -0.0 terms give +0.0)
-__device__ __forceinline__ double dot3(V3 a, V3 b) {
+__host__ __device__ __forceinline__ double dot3(V3 a, V3 b) {
   return dadd(dadd(dadd(0.0, dmul(a.x, b.x)), dmul(a.y, b.y)), dmul(a.z, b.z));
 }
-__device__ __forceinline__ double norm3(V3 a) { return __dsqrt_rn(dot3(a, a)); }
-__device__ __forceinline__ V3 cross3(V3 a, V3 b) {           // Math/Vector.h:1738-1743
+__host__ __device__ __forceinline__ double norm3(V3 a) { return dsqrt(dot3(a, a)); }
+__host__ __device__ __forceinline__ V3 cross3(V3 a, V3 b) {           // Math/Vector.h:1738-1743
   return V3{dsub(dmul(a.y, b.z), dmul(a.z, b.y)), dsub(dmul(a.z, b.x), dmul(a.x, b.z)), dsub(dmul(a.x, b.y), dmul(a.y, b.x))};
 }
 
@@ -65,7 +78,7 @@ __device__ __forceinline__ void tsai_undistort(const TriCam& c, double* px, doub
     double f0, f1;
     tsai_distort(c.k, X0, X1, &f0, &f1);
     const double F0 = dsub(f0, dx), F1 = dsub(f1, dy);
-    const double nf = __dsqrt_rn(dadd(dadd(0.0, dmul(F0, F0)), dmul(F1, F1)));
+    const double nf = dsqrt(dadd(dadd(0.0, dmul(F0, F0)), dmul(F1, F1)));
     if (isnan(nf)) break;
     if (nf < best) { best = nf; B0 = X0; B1 = X1; }
     double J[4];
@@ -75,7 +88,7 @@ __device__ __forceinline__ void tsai_undistort(const TriCam& c, double* px, doub
     const double D0 = ddiv(dsub(dmul(J[3], F0), dmul(J[1], F1)), det);
     const double D1 = ddiv(dsub(dmul(J[0], F1), dmul(J[2], F0)), det);
     X0 = dsub(X0, D0); X1 = dsub(X1, D1);
-    if (__dsqrt_rn(dadd(dadd(0.0, dmul(D0, D0)), dmul(D1, D1))) < 1e-9) { done = true; break; }
+    if (dsqrt(dadd(dadd(0.0, dmul(D0, D0)), dmul(D1, D1))) < 1e-9) { done = true; break; }
   }
   const double U0 = done ? X0 : B0, U1 = done ? X1 : B1;
   *px = dadd(dmul(U0, c.fu), c.cu);
