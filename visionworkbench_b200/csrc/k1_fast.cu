@@ -227,8 +227,8 @@ __device__ __forceinline__ void fast_pass(const uint16_t* __restrict__ ltile, co
                                           uint32_t* __restrict__ best, unsigned long long* __restrict__ keys,
                                           int lane, int g, int ky, int ring_slots, int rw, int ring_base, int idx_base, int nrows, int nb) {
   int V[8][F_B];
-  // Row pointers: the left rows advance by 256, the right rows by rw and wrap around the ring with one compare and
-  // subtract, so a row step computes no slot * rw.
+  // Row pointers: the left rows advance by 256, the right rows by rw and wrap around the ring, so a row step computes no
+  // slot * rw.  The seed wraps rnew before each load, so rnew may sit at rend after it, to be wrapped at the first cut.
   const uint16_t* lnew = ltile + 8 * lane;                      // left row y + ky - 1  (16-byte aligned)
   const uint16_t* lold = lnew;                                  // left row y - 1
   const uint16_t* const rring_lane = rring + 8 * (lane + g);
@@ -242,6 +242,7 @@ __device__ __forceinline__ void fast_pass(const uint16_t* __restrict__ ltile, co
 #pragma unroll
     for (int b = 0; b < F_B; ++b) V[a][b] = 0;
   for (int t = 0; t < ky; ++t) {
+    if (rnew == rend) rnew -= rspan;
     int Lv[8], Rv[16];
     load_row<true>(lnew, rnew, Lv, Rv);
 #pragma unroll
@@ -249,42 +250,10 @@ __device__ __forceinline__ void fast_pass(const uint16_t* __restrict__ ltile, co
 #pragma unroll
       for (int b = 0; b < F_B; ++b) V[a][b] = __sad(Lv[a], Rv[a + b], V[a][b]);
     lnew += F_COLS;
-    rnew += rw; if (rnew == rend) rnew -= rspan;
+    rnew += rw;
   }
-  uint32_t* brow = best + lane;
-  // row y = 0 has no sliding update; the loop leaves after the arg-best of its last row, so the update of every
-  // following row needs no test of y
-  for (int y = 0;;) {
-    // ---- horizontal window sums + min over the 8 dx (keys = cost*8 + b) ----
-    int m[8];
-#pragma unroll
-    for (int b = 0; b < F_B; ++b) {
-      if (!FULL && b >= nb) break;      // last octet of a search width that is not a multiple of 8 (warp uniform)
-      int p[8], o[8];
-      p[0] = V[0][b];
-#pragma unroll
-      for (int a = 1; a < 8; ++a) p[a] = p[a - 1] + V[a][b];
-      window_sums<KX>(p, o);
-#pragma unroll
-      for (int r = 0; r < 8; ++r) m[r] = (b == 0) ? o[r] : min(o[r] + b, m[r]);
-    }
-    // ---- running best: high words hold cost*8 | 7, so m <= s <=> cost <= best cost.  Equal costs are candidates
-    //      too: another warp may hold the same cost at a later disparity ----
-    bool cand = false;
-#pragma unroll
-    for (int r = 0; r < 8; ++r) cand |= ((uint32_t)m[r] <= brow[r * 32]);
-    if (cand) {                // rare once the search has seen the neighbourhood of the true match
-      // The thresholds are read again (volatile), so the common path keeps one predicate rather than eight.  A threshold
-      // lowered meanwhile by another warp only holds back an offer that could not win.
-      const volatile uint32_t* vrow = brow;
-      unsigned long long* krow = keys + y * F_COLS + lane;
-#pragma unroll
-      for (int r = 0; r < 8; ++r)
-        if ((uint32_t)m[r] <= vrow[r * 32]) offer_key(brow + r * 32, krow + r * 32, (uint32_t)m[r] | 7u, (uint32_t)(idx_base + (m[r] & 7)));
-    }
-    if (++y == nrows) break;
-    brow += F_COLS;
-    // ---- slide the vertical sums down one row: + row y + ky - 1, - row y - 1 ----
+  // ---- slide the vertical sums down to row y: + row y + ky - 1, - row y - 1 ----
+  auto slide = [&]() {
     {
       int Lv[8], Rv[16];
       load_row<true>(lnew, rnew, Lv, Rv);
@@ -302,8 +271,67 @@ __device__ __forceinline__ void fast_pass(const uint16_t* __restrict__ ltile, co
         for (int b = 0; b < F_B; ++b) V[a][b] -= __sad(Lo[a], Ro[a + b], 0);
     }
     lnew += F_COLS; lold += F_COLS;
-    rnew += rw; if (rnew == rend) rnew -= rspan;
-    rold += rw; if (rold == rend) rold -= rspan;
+    rnew += rw; rold += rw;
+  };
+  // The pass reads nrows + ky - 1 <= ring_slots consecutive ring rows, so each right pointer wraps at most once: rnew
+  // before the slide to row ynew, rold (ky rows behind) before the slide to row yold.  Rows between those cuts run in
+  // one inner loop whose pointers advance without a test.
+  const int ynew = ring_slots - ring_base - ky + 1, yold = ynew + ky;
+  uint32_t* brow = best + lane;
+  // row y = 0 has no sliding update; the inner loop leaves after the arg-best of its last row, so the update of every
+  // following row needs no test of y
+  for (int y = 0;;) {
+    const int yend = min(nrows, y < ynew ? ynew : y < yold ? yold : nrows);
+    for (;;) {
+      // ---- horizontal window sums + min over the 8 dx (keys = cost*8 + b) ----
+      int m[8];
+      if (FULL) {
+        // dx b and b + 4 together: two independent prefix / shuffle / add chains (the keys make the min order-free)
+#pragma unroll
+        for (int b = 0; b < F_B / 2; ++b) {
+          int p0[8], p1[8], o0[8], o1[8];
+          p0[0] = V[0][b]; p1[0] = V[0][b + 4];
+#pragma unroll
+          for (int a = 1; a < 8; ++a) { p0[a] = p0[a - 1] + V[a][b]; p1[a] = p1[a - 1] + V[a][b + 4]; }
+          window_sums2<KX>(p0, p1, o0, o1);
+#pragma unroll
+          for (int r = 0; r < 8; ++r) m[r] = min(o1[r] + b + 4, (b == 0) ? o0[r] : min(o0[r] + b, m[r]));
+        }
+      } else {
+#pragma unroll
+        for (int b = 0; b < F_B; ++b) {
+          if (b >= nb) break;               // last octet of a search width that is not a multiple of 8 (warp uniform)
+          int p[8], o[8];
+          p[0] = V[0][b];
+#pragma unroll
+          for (int a = 1; a < 8; ++a) p[a] = p[a - 1] + V[a][b];
+          window_sums<KX>(p, o);
+#pragma unroll
+          for (int r = 0; r < 8; ++r) m[r] = (b == 0) ? o[r] : min(o[r] + b, m[r]);
+        }
+      }
+      // ---- running best: high words hold cost*8 | 7, so m <= s <=> cost <= best cost.  Equal costs are candidates
+      //      too: another warp may hold the same cost at a later disparity ----
+      bool cand = false;
+#pragma unroll
+      for (int r = 0; r < 8; ++r) cand |= ((uint32_t)m[r] <= brow[r * 32]);
+      if (cand) {                // rare once the search has seen the neighbourhood of the true match
+        // The thresholds are read again (volatile), so the common path keeps one predicate rather than eight.  A threshold
+        // lowered meanwhile by another warp only holds back an offer that could not win.
+        const volatile uint32_t* vrow = brow;
+        unsigned long long* krow = keys + y * F_COLS + lane;
+#pragma unroll
+        for (int r = 0; r < 8; ++r)
+          if ((uint32_t)m[r] <= vrow[r * 32]) offer_key(brow + r * 32, krow + r * 32, (uint32_t)m[r] | 7u, (uint32_t)(idx_base + (m[r] & 7)));
+      }
+      brow += F_COLS;
+      if (++y == yend) break;
+      slide();
+    }
+    if (y == nrows) break;
+    if (y == ynew) rnew -= rspan;
+    if (y == yold) rold -= rspan;
+    slide();
   }
 }
 

@@ -113,5 +113,44 @@ __device__ __forceinline__ void window_sums(const int (&p)[8], int (&out)[8]) {
   }
 }
 
+// window_sums of two independent prefix rows (two dx of an octet), the same outputs: every shuffle of both is issued
+// before the adds that consume them, so each batch of shuffles has two chains to overlap instead of one.
+template <int KX>
+__device__ __forceinline__ void window_sums2(const int (&p0)[8], const int (&p1)[8], int (&o0)[8], int (&o1)[8]) {
+  constexpr int MAXL = (KX - 1) / 8;
+  int t0[MAXL + 1], t1[MAXL + 1], q0[8], q1[8];
+#pragma unroll
+  for (int k = 1; k <= MAXL; ++k) {
+    t0[k] = __shfl_down_sync(0xffffffffu, p0[7], k);
+    t1[k] = __shfl_down_sync(0xffffffffu, p1[7], k);
+  }
+#pragma unroll
+  for (int r = 0; r < 8; ++r) {
+    const int rem = KX - (8 - r), full = rem / 8, part = rem % 8;
+    if (rem > 0 && part) {
+      q0[r] = __shfl_down_sync(0xffffffffu, p0[part - 1], full + 1);
+      q1[r] = __shfl_down_sync(0xffffffffu, p1[part - 1], full + 1);
+    }
+  }
+  int W0[MAXL + 1], W1[MAXL + 1];
+  W0[0] = p0[7]; W1[0] = p1[7];
+#pragma unroll
+  for (int k = 1; k <= MAXL; ++k) { W0[k] = W0[k - 1] + t0[k]; W1[k] = W1[k - 1] + t1[k]; }
+#pragma unroll
+  for (int r = 0; r < 8; ++r) {
+    const int rem = KX - (8 - r), full = rem / 8, part = rem % 8;
+    if (rem <= 0) {
+      o0[r] = r ? p0[r + KX - 1] - p0[r - 1] : p0[KX - 1];
+      o1[r] = r ? p1[r + KX - 1] - p1[r - 1] : p1[KX - 1];
+    } else if (part) {
+      o0[r] = r ? (W0[full] + q0[r]) - p0[r - 1] : W0[full] + q0[r];
+      o1[r] = r ? (W1[full] + q1[r]) - p1[r - 1] : W1[full] + q1[r];
+    } else {
+      o0[r] = r ? W0[full] - p0[r - 1] : W0[full];
+      o1[r] = r ? W1[full] - p1[r - 1] : W1[full];
+    }
+  }
+}
+
 
 }  // namespace vwb200
