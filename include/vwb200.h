@@ -589,6 +589,35 @@ int  vwb200_shard_exchange_halos(vwb200_shard* s, const vwb200_band_plan* plan, 
                                  float* right_band, int rcols, ptrdiff_t rpitch, void* stream);
 void vwb200_shard_destroy(vwb200_shard* s);
 
+/* ---- a20 / K12: interest point detection and description (ipfind --interest-operator iagd, sgrad descriptor) -----------
+ * Rasters are single-channel float (pitches in floats), in host or device memory (on_device), on `stream`.  Point lists are
+ * host arrays of vwb200_ip_point.  Every call is bit for bit the reference's (tools/ipfind.cc:253-401):
+ *  - normalize: normalize(image), or with has_nodata apply_mask(normalize(create_mask(image, nodata))) (min / max of the
+ *    pixels != (float)nodata; those pixels become 0).  NaN or +-inf anywhere, or no valid pixel, is VWB200_EARG.
+ *  - detect: detect_interest_points(image, IntegralAutoGainDetector(ip_per_tile), ip_per_tile) with default_tile_size
+ *    tile_size (detection tiles are max(1024, tile_size) square).  ip_per_tile 0 keeps every point.  At most cap points are
+ *    written; *n receives the count, and a count above cap is VWB200_EARG (call again with cap >= *n).
+ *  - remove_near_nodata: remove_ip_near_nodata(raw, nodata, list, radius) in place (*n in: count, out: kept).
+ *  - describe: describe_interest_points(image, SGradDescriptorGenerator, list): the list is reordered as its per-tile
+ *    std::partition does, x / y take the crop round trip's rounding, and desc receives n * 180 floats in the new order.
+ *    cos / sin of -orientation are taken on the host with the C library.  A point whose (int)x, (int)y lies outside the
+ *    image is VWB200_EARG. */
+typedef struct { float x, y; int32_t ix, iy; float scale, interest, orientation; } vwb200_ip_point;
+int vwb200_ipfind_normalize(const float* in, int w, int h, ptrdiff_t pitch, int has_nodata, double nodata, float* out, ptrdiff_t out_pitch,
+                            int on_device, void* stream);
+int vwb200_ipfind_detect(const float* image, int w, int h, ptrdiff_t pitch, int tile_size, int ip_per_tile, vwb200_ip_point* out,
+                         long long cap, long long* n, int on_device, void* stream);
+int vwb200_ipfind_remove_near_nodata(const float* raw, int w, int h, ptrdiff_t pitch, double nodata, int radius, vwb200_ip_point* pts,
+                                     long long* n, int on_device, void* stream);
+int vwb200_ipfind_describe(const float* image, int w, int h, ptrdiff_t pitch, int tile_size, vwb200_ip_point* pts, long long n,
+                           float* desc, int on_device, void* stream);
+/* generate_gaussian_kernel(k, 2, 9): the Harris taps the detector weights by (host, no device needed) */
+int vwb200_ipfind_gaussian_taps(double* k9);
+/* the last detect / describe on this thread: tiles, raw extrema, points kept after the auto-gain and Harris thresholds,
+ * tiles culled to their num_ip, and points described */
+typedef struct { long long tiles, extrema, kept, culled_tiles, described; } vwb200_ipfind_stats;
+int vwb200_last_ipfind_stats(vwb200_ipfind_stats* out);
+
 /* Scratch memory is stream-ordered and stays cached in the device's default memory pool between calls (returning it at
  * every synchronisation costs ~100 ms per 8K x 8K call).  vwb200_trim() hands the cached memory back to the driver. */
 int vwb200_trim(void);

@@ -32,6 +32,7 @@ the library or a CUDA device is missing.  Inputs may be numpy arrays (staged thr
 library) or torch CUDA tensors (used in place, results returned as torch CUDA tensors).
 """
 import ctypes as C
+import math
 import os
 import re
 
@@ -1458,3 +1459,196 @@ def read_binary_match_file(path):
     ip1, off = _read_records(buf, 16, n1)
     ip2, _ = _read_records(buf, off, n2)
     return ip1, ip2
+
+
+# ---- a20 / K12: interest point detection and description (ipfind --interest-operator iagd, sgrad descriptor) ----------
+class IpPoint(C.Structure):
+    _fields_ = [("x", C.c_float), ("y", C.c_float), ("ix", C.c_int32), ("iy", C.c_int32), ("scale", C.c_float),
+                ("interest", C.c_float), ("orientation", C.c_float)]
+
+
+class IpfindStats(C.Structure):
+    _fields_ = [("tiles", C.c_longlong), ("extrema", C.c_longlong), ("kept", C.c_longlong), ("culled_tiles", C.c_longlong),
+                ("described", C.c_longlong)]
+
+
+_IPF_POINT = np.dtype([("x", "<f4"), ("y", "<f4"), ("ix", "<i4"), ("iy", "<i4"), ("scale", "<f4"), ("interest", "<f4"),
+                       ("orientation", "<f4")])
+_IPF_READY = False
+_IPF_EARG = -1                                  # vwb200_ipfind_detect: more points than cap (*n holds the count)
+SGRAD_SIZE = 180
+
+
+def _ipf():
+    global _IPF_READY
+    L = lib()
+    if not _IPF_READY:
+        P, I, Z, LL = C.c_void_p, C.c_int, C.c_ssize_t, C.c_longlong
+        L.vwb200_ipfind_normalize.argtypes = [P, I, I, Z, I, C.c_double, P, Z, I, P]
+        L.vwb200_ipfind_detect.argtypes = [P, I, I, Z, I, I, P, LL, C.POINTER(LL), I, P]
+        L.vwb200_ipfind_remove_near_nodata.argtypes = [P, I, I, Z, C.c_double, I, P, C.POINTER(LL), I, P]
+        L.vwb200_ipfind_describe.argtypes = [P, I, I, Z, I, P, LL, P, I, P]
+        L.vwb200_ipfind_gaussian_taps.argtypes = [P]
+        L.vwb200_last_ipfind_stats.argtypes = [C.POINTER(IpfindStats)]
+        _IPF_READY = True
+    return L
+
+
+def _image2d(image, what):
+    if not _is_torch(image) and _np(image, np.float32).ndim != 2:
+        raise ArgumentErr(f"{what}: the image must be 2-D")
+    return _raster(image, np.float32)
+
+
+def _ipf_points(points):
+    """the vwb200_ip_point array of an interest_points() record array (or of any array with x, y fields)"""
+    rec = np.asarray(points)
+    p = np.zeros(len(rec), _IPF_POINT)
+    names = rec.dtype.names or ()
+    if "x" not in names or "y" not in names:
+        raise ArgumentErr("points need x and y fields")
+    p["x"], p["y"] = rec["x"], rec["y"]
+    p["ix"] = rec["ix"] if "ix" in names else rec["x"].astype(np.float32).astype(np.int32)
+    p["iy"] = rec["iy"] if "iy" in names else rec["y"].astype(np.float32).astype(np.int32)
+    p["scale"] = rec["scale"] if "scale" in names else 1.0
+    for f in ("interest", "orientation"):
+        if f in names:
+            p[f] = rec[f]
+    return p
+
+
+def _ipf_records(p, descriptor=None, base=None):
+    """an interest_points() record array of vwb200_ip_point p (the other fields from `base`, in p's order, or their defaults)"""
+    d = np.zeros((len(p), 0), np.float32) if descriptor is None else np.asarray(descriptor, np.float32)
+    rec = np.zeros(len(p), _ip_dtype(d.shape[1]))
+    for f in ("x", "y", "ix", "iy", "scale", "interest", "orientation"):
+        rec[f] = p[f]
+    rec["size"] = d.shape[1]
+    rec["descriptor"] = d
+    if base is not None:
+        for f in ("polarity", "octave", "scale_lvl"):
+            rec[f] = base[f]
+    return rec
+
+
+def normalize(image, nodata=None):
+    """normalize(image) to [0, 1] (Image/AutoNormalize.h:76-86), or with nodata apply_mask(normalize(create_mask(image,
+    nodata))): the min / max are those of the pixels != float32(nodata), which become 0.  NaN / inf anywhere, or no valid
+    pixel, is ArgumentErr.  Returns a new float32 raster where the image lives."""
+    t, ptr, cols, rows, pitch, dev = _image2d(image, "normalize")
+    out = _output(t, (rows, cols), np.float32)
+    _check(_ipf().vwb200_ipfind_normalize(ptr, cols, rows, pitch, nodata is not None, 0.0 if nodata is None else float(nodata), _ptr(out),
+                                          cols, dev, _stream_ptr() if dev else None))
+    return out
+
+
+def ipfind_gaussian_taps():
+    """generate_gaussian_kernel(k, 2, 9): the nine Harris taps of the detector (float64)"""
+    k = np.zeros(9, np.float64)
+    _check(_ipf().vwb200_ipfind_gaussian_taps(k.ctypes.data))
+    return k
+
+
+def detection_tile_count(cols, rows, tile_size=1024):
+    ts = max(1024, int(tile_size))
+    return (-(-cols // ts)) * (-(-rows // ts)) if cols > 0 and rows > 0 else 0
+
+
+def tile_num_ip(tile_w, tile_h, ip_per_tile, tile_size=1024):
+    """InterestDetectionQueue's per-tile count (DetectorBase.h:276-290): clamp(ceil(area / tile^2 * desired), 1, desired);
+    0 (keep every point) when ip_per_tile is 0"""
+    if ip_per_tile <= 0:
+        return 0
+    ts = max(1024, int(tile_size))
+    return max(1, min(int(math.ceil(float(tile_w) * tile_h / (float(ts) * ts) * float(ip_per_tile))), int(ip_per_tile)))
+
+
+def ip_per_tile_for_image(ip_per_image, cols, rows, tile_size=1024):
+    """ipfind.cc:255-262: max(1, ceil(ip_per_image / (cols * rows / tile_size^2))) with the unclamped tile_size"""
+    num_tiles = cols * rows / float(tile_size * tile_size)
+    return max(1, int(math.ceil(ip_per_image / num_tiles)))
+
+
+def detect_interest_points_iagd(image, ip_per_tile=250, tile_size=1024):
+    """detect_interest_points(image, IntegralAutoGainDetector(ip_per_tile), ip_per_tile) (InterestPoint/DetectorBase.h:250-328,
+    IntegralDetector.cc:264-370) on a float32 image, numpy or CUDA, usually normalize()'s output.  tile_size is the default
+    tile size (tiles are max(1024, tile_size) square); ip_per_tile 0 keeps every point.  Returns an interest_points() array
+    with empty descriptors, in the reference's order."""
+    if ip_per_tile < 0:
+        raise ArgumentErr("detect_interest_points_iagd: ip_per_tile must be >= 0")
+    t, ptr, cols, rows, pitch, dev = _image2d(image, "detect_interest_points_iagd")
+    ntiles = detection_tile_count(cols, rows, tile_size)
+    cap = ntiles * int(ip_per_tile) if ip_per_tile > 0 else max(4096, cols * rows // 64)
+    n = C.c_longlong()
+    while True:
+        p = np.zeros(max(cap, 1), _IPF_POINT)
+        rc = _ipf().vwb200_ipfind_detect(ptr, cols, rows, pitch, int(tile_size), int(ip_per_tile), p.ctypes.data, cap, C.byref(n), dev,
+                                         _stream_ptr() if dev else None)
+        if rc == _IPF_EARG and n.value > cap:
+            cap = n.value
+            continue
+        _check(rc)
+        break
+    return _ipf_records(p[:n.value])
+
+
+
+def remove_ip_near_nodata(raw_image, points, nodata=0.0, radius=1):
+    """remove_ip_near_nodata(raw, nodata, list, radius) (InterestPoint/InterestPointUtils.h:45-82): drops the points whose
+    (ix, iy) lies within radius of the image border or whose (2 radius + 1)^2 window holds a pixel equal to nodata (compared
+    in double).  Returns the kept records of `points`, in order."""
+    rec = np.asarray(points)
+    p = _ipf_points(rec)
+    t, ptr, cols, rows, pitch, dev = _image2d(raw_image, "remove_ip_near_nodata")
+    n = C.c_longlong(len(p))
+    idx = np.arange(len(p), dtype=np.int32)
+    p["interest"] = idx.view(np.float32)          # carry each point's index through the compaction
+    _check(_ipf().vwb200_ipfind_remove_near_nodata(ptr, cols, rows, pitch, float(nodata), int(radius), p.ctypes.data, C.byref(n), dev,
+                                                   _stream_ptr() if dev else None))
+    return rec[p["interest"][:n.value].view(np.int32)].copy()
+
+
+def describe_sgrad(image, points, tile_size=1024):
+    """describe_interest_points(image, SGradDescriptorGenerator, list) (InterestPoint/Descriptor.h:202-355, 414-471) on a
+    float32 image, numpy or CUDA: the list is reordered as the reference's per-tile std::partition does, x / y take its crop
+    round trip's float rounding, and each point gets the 180-float SGrad descriptor.  Returns a new interest_points() array."""
+    rec = np.asarray(points)
+    p = _ipf_points(rec)
+    p_idx = np.arange(len(p), dtype=np.int32)
+    t, ptr, cols, rows, pitch, dev = _image2d(image, "describe_sgrad")
+    desc = np.zeros((len(p), SGRAD_SIZE), np.float32)
+    # the partition moves whole points: order the extra fields by matching each output point back by its index
+    q = p.copy()
+    q["ix"] = p_idx
+    _check(_ipf().vwb200_ipfind_describe(ptr, cols, rows, pitch, int(tile_size), q.ctypes.data, len(q), desc.ctypes.data, dev,
+                                         _stream_ptr() if dev else None))
+    order = q["ix"].copy()
+    q["ix"] = p["ix"][order]
+    base = rec[order] if rec.dtype.names and "polarity" in rec.dtype.names else None
+    return _ipf_records(q, desc, base)
+
+
+def last_ipfind_stats():
+    """what the last detect_interest_points_iagd / describe_sgrad on this thread did: tiles, raw extrema, points kept after
+    the auto-gain and Harris thresholds, tiles culled to their num_ip, points described"""
+    s = IpfindStats()
+    _ipf().vwb200_last_ipfind_stats(C.byref(s))
+    return {f: int(getattr(s, f)) for f, _ in IpfindStats._fields_}
+
+
+def ipfind(image, ip_per_tile=250, ip_per_image=0, nodata=None, nodata_radius=1, tile_size=1024, no_orientation=False):
+    """ipfind --interest-operator iagd (tools/ipfind.cc:253-401): normalize, detect, remove the points near nodata (0 when
+    nodata is None, as ipfind does) when nodata_radius > 0, then the sgrad descriptor.  Returns an interest_points() array
+    whose write_binary_ip_file bytes are ipfind's .vwip."""
+    t, ptr, cols, rows, pitch, dev = _image2d(image, "ipfind")
+    if ip_per_image > 0:
+        ip_per_tile = ip_per_tile_for_image(ip_per_image, cols, rows, tile_size)
+    img = normalize(image, nodata)
+    pts = detect_interest_points_iagd(img, ip_per_tile, tile_size)
+    if len(pts) == 0:
+        return _ipf_records(np.zeros(0, _IPF_POINT), np.zeros((0, SGRAD_SIZE), np.float32))
+    if nodata_radius > 0:
+        pts = remove_ip_near_nodata(image, pts, 0.0 if nodata is None else nodata, nodata_radius)
+    if no_orientation:
+        pts["orientation"] = 0
+    return describe_sgrad(img, pts, tile_size)

@@ -10,7 +10,7 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(ROOT, "build", "obj")
 SO = os.path.join(HERE, "libvwb200.so")
-SOURCES = ["engine.cu", "cameras.cu", "k1_generic.cu", "k1_zone_int.cu", "k1_fast.cu", "k1_screen.cu", "k2_pyramid.cu", "k34_filters.cu", "k5_sgm.cu", "k5_sgm_paths.cu", "k6_smoothing.cu", "k7_dispmap.cu", "k8_warp.cu", "k9_inpaint.cu", "k10_triangulate.cu", "k11_ipmatch.cu", "shard.cu"]
+SOURCES = ["engine.cu", "cameras.cu", "k1_generic.cu", "k1_zone_int.cu", "k1_fast.cu", "k1_screen.cu", "k2_pyramid.cu", "k34_filters.cu", "k5_sgm.cu", "k5_sgm_paths.cu", "k6_smoothing.cu", "k7_dispmap.cu", "k8_warp.cu", "k9_inpaint.cu", "k10_triangulate.cu", "k11_ipmatch.cu", "k12_ipfind.cu", "shard.cu"]
 # -ffp-contract=off: the host camera math (cameras.cu, with pinhole.cuh / cahv.cuh) rounds every product and sum as the
 # reference does, never fused into an FMA; the device side uses explicitly rounded intrinsics instead
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
